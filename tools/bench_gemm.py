@@ -1,7 +1,9 @@
 #!/usr/bin/env python
-"""Times the wgmma GEMM family alone on the shapes of the b128 train step (M = 131072 tokens, d = 512, FFN inner 1365 -> 1408 / 2816).
-TFX_LIB=<path to a libtfx_b200 build> selects a library variant (A/B experiments)."""
-import os, sys
+"""Times the wgmma GEMM family alone on the shapes of the b128 train step (M = 131072 tokens, d = 512, heads 8, FFN inner 1365 -> 1408 / 2816).
+TFX_LIB=<path to a libtfx_b200 build> selects a library variant (A/B experiments).  --dump DIR writes each case's outputs as
+DIR/<case>.<tensor>.npy, so that two builds can be compared bit for bit (split-K cases accumulate with atomics and are not written)."""
+import argparse, os, sys
+import numpy as np
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from transfusion_pytorch_b200 import _lib
@@ -9,24 +11,57 @@ if os.environ.get('TFX_LIB'):
     _lib.LIB_PATH = os.environ['TFX_LIB']
 
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--dump', default = None, metavar = 'DIR', help = 'write the outputs of every non-split-K case to DIR/*.npy')
+    args = ap.parse_args()
     ops = _lib.Ops()
-    M, D, Ip = int(os.environ.get('TOKENS', 131072)), 512, 1408
+    M, D, Ip, H = int(os.environ.get('TOKENS', 131072)), 512, 1408, 8
+    HI, NQ, n_cond = H * 64, 3 * H * 64 + 128, 128
     bf = torch.bfloat16
-    r = lambda *s: (torch.randn(*s, device = 'cuda') * 0.05).to(bf)
+    g = torch.Generator(device = 'cuda').manual_seed(0)
+    r = lambda *s: (torch.randn(*s, device = 'cuda', generator = g) * 0.05).to(bf)
     u, w1, b1 = r(M, D), r(2 * Ip, D), torch.zeros(2 * Ip, device = 'cuda')
     vg, h = torch.empty(M, 2 * Ip, device = 'cuda', dtype = bf), torch.empty(M, Ip, device = 'cuda', dtype = bf)
     w2 = r(D, Ip); dy = r(M, D); dh = torch.empty(M, Ip, device = 'cuda', dtype = bf); du = torch.empty(M, D, device = 'cuda', dtype = bf)
     gw = torch.zeros(2 * Ip, D, device = 'cuda')
-    cases = {
-        'geglu  [131072 x 2816 x 512]': (lambda: ops.gemm_geglu(u, D, w1, D, b1, M, 2 * Ip, D, vg, h), 2.0 * M * 2 * Ip * D),
-        'store  [131072 x 2816 x 512]': (lambda: ops.gemm_store(u, D, 0, w1, D, 0, M, 2 * Ip, D, None, 0, vg, 2 * Ip, None, None, 1.0, 0, 1), 2.0 * M * 2 * Ip * D),
-        'dgrad  [131072 x 1408 x 512]': (lambda: ops.gemm_store(dy, D, 0, w2, Ip, 1, M, Ip, D, None, 0, dh, Ip, None, None, 1.0, 0, 1), 2.0 * M * Ip * D),
-        'dgrad  [131072 x 512 x 2816]': (lambda: ops.gemm_store(vg, 2 * Ip, 0, w1, D, 1, M, D, 2 * Ip, None, 0, du, D, None, None, 1.0, 0, 1), 2.0 * M * 2 * Ip * D),
-        'wgrad  [2816 x 512 x 131072]': (lambda: ops.gemm_store(vg, 2 * Ip, 1, u, D, 1, 2 * Ip, D, M, gw, D, None, 0, None, None, 1.0, 1, 20), 2.0 * M * 2 * Ip * D),
+    # QKVG: to_qk | to_v | to_gates (2 heads per 128-column tile) + qk-RMSNorm + RoPE
+    wq = r(NQ, D)
+    q, k, v = (torch.empty(M, HI, device = 'cuda', dtype = bf) for _ in range(3))
+    gates, qk_inv = torch.empty(M, H, device = 'cuda'), torch.empty(M, 2 * H, device = 'cuda')
+    gq, gk = (torch.randn(64, device = 'cuda', generator = g) * 0.3 for _ in range(2))
+    pos = (torch.arange(M, device = 'cuda') % 1024).to(torch.int32)             # positions of packed 1024-token sequences
+    freqs = 1. / (10000 ** (torch.arange(0, 64, 2, device = 'cuda').float() / 64))
+    rope_t, rope_tt = torch.empty(1024, 32, 2, device = 'cuda'), torch.empty(32, 1024, 2, device = 'cuda')
+    ops.rope_table(freqs, rope_t, rope_tt, 1024, 32)
+    # RESID as the engine calls it: to_out (fp32 residual in / out, bf16 branch output saved) and ffn_out (bf16 hidden state out)
+    att, wo, w2r = r(M, HI), r(D, HI), r(D, Ip)
+    bias2 = torch.randn(D, device = 'cuda', generator = g) * 0.1
+    x_a = torch.randn(M, D, device = 'cuda', generator = g)
+    x_b, x_cb = torch.empty(M, D, device = 'cuda'), torch.empty(M, D, device = 'cuda', dtype = bf)
+    yA, yF = (torch.empty(M, D, device = 'cuda', dtype = bf) for _ in range(2))
+    cond_row = torch.randint(-1, n_cond, (M,), device = 'cuda', generator = g, dtype = torch.int32)
+    zg = torch.rand(n_cond, 2 * D, device = 'cuda', generator = g)
+    ls = torch.randn(D, device = 'cuda', generator = g) * 0.1
+    cases = {   # name: (launch, algorithmic FLOPs, outputs to dump)
+        'qkvg   [131072 x 1664 x 512]': (lambda: ops.gemm_qkvg(u, D, wq, D, M, H, D, q, k, v, gates, qk_inv, gq, gk, pos, rope_tt, 1024, None, None),
+                                         2.0 * M * NQ * D, dict(q = q, k = k, v = v, gates = gates, qk_inv = qk_inv)),
+        'resid  [131072 x 512 x 512]': (lambda: ops.gemm_resid(att, HI, None, 0, 0, wo, HI, M, D, HI, None, x_a, x_b, None, yA, cond_row, zg[:, D:], 2 * D, ls),
+                                        2.0 * M * D * HI, dict(x_out = x_b, y = yA)),
+        'resid  [131072 x 512 x 1408]': (lambda: ops.gemm_resid(h, Ip, None, 0, 0, w2r, Ip, M, D, Ip, bias2, x_b, None, x_cb, yF, cond_row, zg[:, :D], 2 * D, ls),
+                                         2.0 * M * D * Ip, dict(x_out_bf16 = x_cb, y = yF)),
+        'geglu  [131072 x 2816 x 512]': (lambda: ops.gemm_geglu(u, D, w1, D, b1, M, 2 * Ip, D, vg, h), 2.0 * M * 2 * Ip * D, dict(vg = vg, h = h)),
+        'store  [131072 x 2816 x 512]': (lambda: ops.gemm_store(u, D, 0, w1, D, 0, M, 2 * Ip, D, None, 0, vg, 2 * Ip, None, None, 1.0, 0, 1), 2.0 * M * 2 * Ip * D,
+                                         dict(out = vg)),
+        'dgrad  [131072 x 1408 x 512]': (lambda: ops.gemm_store(dy, D, 0, w2, Ip, 1, M, Ip, D, None, 0, dh, Ip, None, None, 1.0, 0, 1), 2.0 * M * Ip * D, dict(out = dh)),
+        'dgrad  [131072 x 512 x 2816]': (lambda: ops.gemm_store(vg, 2 * Ip, 0, w1, D, 1, M, D, 2 * Ip, None, 0, du, D, None, None, 1.0, 0, 1), 2.0 * M * 2 * Ip * D,
+                                         dict(out = du)),
+        'wgrad  [2816 x 512 x 131072]': (lambda: ops.gemm_store(vg, 2 * Ip, 1, u, D, 1, 2 * Ip, D, M, gw, D, None, 0, None, None, 1.0, 1, 20), 2.0 * M * 2 * Ip * D, {}),
     }
     big = torch.empty(256 << 20, dtype = torch.uint8, device = 'cuda')
     tag = os.path.basename(os.environ.get('TFX_LIB', 'default'))
-    for name, (fn, fl) in cases.items():
+    if args.dump:
+        os.makedirs(args.dump, exist_ok = True)
+    for name, (fn, fl, outs) in cases.items():
         for _ in range(3): fn()
         ts = []
         for _ in range(10):
@@ -36,5 +71,10 @@ def main():
             ts.append(e0.elapsed_time(e1) * 1e3)
         med = sorted(ts)[5]
         print(f'{tag:36s} {name}: median {med:8.1f} us  min {min(ts):8.1f} us  {fl / med / 1e6:7.1f} TFLOP/s')
+        if args.dump:
+            case = name.split()[0] + '_' + name.split('[')[1].rstrip(']').replace(' x ', 'x')
+            for tn, t in outs.items():
+                a = t.cpu()
+                np.save(os.path.join(args.dump, f'{case}.{tn}.npy'), (a.view(torch.int16) if a.dtype == bf else a).numpy())
 if __name__ == '__main__':
     main()

@@ -1,20 +1,29 @@
-// Persistent, warp-specialised bf16 GEMM for sm_90a: TMA (128B swizzle) -> smem ring -> wgmma (two consumer
-// warpgroups, 64 x 128 x 16 each, fp32 accumulators in registers) -> accumulator tile staged through shared memory
-// -> the Transfusion-specific fused epilogues.
+// Persistent, warp-specialised bf16 GEMM for sm_90a: TMA (128B swizzle) -> smem ring -> wgmma (two consumer warpgroups in
+// ping-pong, each computing whole 128 x 128 tiles with fp32 accumulators in registers) -> accumulator tile staged through
+// shared memory -> the Transfusion-specific fused epilogues.
 //
 //   D[m][n] = sum_k A(m,k) * B(n,k)
 //   A "K-major":  stored row-major [M][K]   (activations as GEMM input, dY for dgrad)
 //   A "MN-major": stored row-major [K][M]   (dY^T for wgrad: K = tokens)
 //   B likewise over n.
 //
-// Roles (384 threads): warpgroup 0 = TMA producer (one lane), warpgroups 1 and 2 = wgmma consumers (rows 0-63 / 64-127 of the
-// 128 x 128 tile) that also run the epilogue.  After a tile's main loop the consumers write their accumulator fragments into a
-// 64 KB fp32 tile in shared memory; each epilogue thread then owns ONE accumulator row (warp e = 0..7 of the consumers: rows
-// 32 (e % 4) .. + 31, column slice e / 4), the layout the per-row epilogue math (qk-RMSNorm, RoPE, gate select) wants.  The
-// producer keeps filling the ring for the next tile while the epilogue runs.
+// Roles (384 threads): warpgroup 0 = TMA producer (one lane, 40 registers), warpgroups 1 and 2 = wgmma consumers (232 registers)
+// that also run the epilogue.  The consumers take alternate work items of the CTA's sequence (j = 0, 2, .. and j = 1, 3, ..), so
+// one warpgroup's epilogue runs while the other's main loop keeps the tensor cores busy.  Per 16-deep k step a consumer issues two
+// wgmma.m64n128k16 (rows 0-63, rows 64-127).  Two hand-offs order the warpgroups, both as named-barrier pairs (one warpgroup
+// arrives, the other waits):
+//   MMA: item j's main loop starts after item j-1's last k-block was issued.  Besides keeping the tensor cores on one tile at a
+//        time, this is what makes the ring's parity waits exact: a consumer skips the other's k-blocks, and without the hand-off it
+//        could wait on a full barrier two phases ahead of the one in flight and take a stale completion for its own.
+//   ACC: item j's accumulators go to the 64 KB fp32 tile in shared memory after item j-1's epilogue has finished with it and with
+//        the staging tiles.  GEGLU reads its whole accumulator row first and hands the tile on right then; its warpgroups stage
+//        through separate tiles, so the GELU math and stores of item j-1 overlap item j's accumulator write.
+// In the epilogue each thread of the warpgroup owns ONE accumulator row (warp q = 0..3: rows 32 q .. + 31, all 128 columns), the
+// layout the per-row epilogue math (qk-RMSNorm, RoPE, gate select) wants.
 //
 // Epilogue global traffic is staged through a per-warp 32 x 128 B shared-memory tile (XOR-swizzled 16 B chunks) so that every
-// global load / store instruction covers whole 64 / 128-byte row segments.
+// global load / store instruction covers whole 64 / 128-byte row segments.  Apart from GEGLU, one warpgroup runs an epilogue at a
+// time, so the two share four such tiles.
 //
 // CL = 2: a cluster of two CTAs computes two vertically adjacent 128 x 128 tiles that share one B tile.  Each CTA loads its own A
 // tile and HALF of the B tile, multicast into the same offset of both CTAs' rings, so a pair reads B from L2 once instead of twice.
@@ -68,14 +77,15 @@ struct GemmParams {
 
 template <int EPI> struct GemmCfg {
   static constexpr int THREADS = 384;
-  static constexpr int STAGES = EPI == 2 ? 3 : 4;
+  static constexpr int STAGES = 4;
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
   static constexpr int B_BYTES = GEMM_BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int ACC_BYTES = GEMM_BM * GEMM_BN * 4;          // fp32 accumulator tile, rows of 512 B
-  // per-warp staging: 32 rows x 128 B; RESID adds a 64-byte-pitch bf16 tile (2 KB)
+  // per-warp staging: 32 rows x 128 B; RESID adds a 64-byte-pitch bf16 tile (2 KB).  Four warps (one epilogue warpgroup at a
+  // time), except GEGLU: its warpgroups hand the accumulator tile over before their epilogues end, so each has its own four.
   static constexpr int STG_WARP = EPI == 2 ? 4096 + 2048 : 4096;
-  static constexpr int STAGING = 8 * STG_WARP;
+  static constexpr int STAGING = (EPI == 3 ? 8 : 4) * STG_WARP;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + STAGING + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one block");
 };
@@ -153,15 +163,20 @@ __device__ __forceinline__ void stg_store(const uint8_t* sw, int lane, uint8_t* 
       *reinterpret_cast<uint4*>(g + row * pitch + ch * 16) = *reinterpret_cast<const uint4*>(sw + row * 128 + ((ch ^ (row & 7)) << 4));
   }
 }
-template <int CH>
-__device__ __forceinline__ void stg_load(uint8_t* sw, int lane, const uint8_t* g, long long pitch, int rows_valid) {
-  constexpr int RPI = 32 / CH;
+// coalesced global load of a 32 x 128 B tile into registers (4 rows per instruction; rows >= rows_valid read as zero), and those
+// registers into the staging tile: split so that the loads of several tiles can be in flight at once
+__device__ __forceinline__ void stg_fetch(int lane, const uint8_t* g, long long pitch, int rows_valid, uint4 (&t)[8]) {
 #pragma unroll
-  for (int it = 0; it < 32 / RPI; ++it) {
-    const int row = it * RPI + lane / CH, ch = lane % CH;
-    uint4 t = make_uint4(0, 0, 0, 0);
-    if (row < rows_valid) t = *reinterpret_cast<const uint4*>(g + row * pitch + ch * 16);
-    *reinterpret_cast<uint4*>(sw + row * 128 + ((ch ^ (row & 7)) << 4)) = t;
+  for (int it = 0; it < 8; ++it) {
+    const int row = it * 4 + lane / 8, ch = lane % 8;
+    t[it] = row < rows_valid ? *reinterpret_cast<const uint4*>(g + row * pitch + ch * 16) : make_uint4(0, 0, 0, 0);
+  }
+}
+__device__ __forceinline__ void stg_fill(uint8_t* sw, int lane, const uint4 (&t)[8]) {
+#pragma unroll
+  for (int it = 0; it < 8; ++it) {
+    const int row = it * 4 + lane / 8, ch = lane % 8;
+    *reinterpret_cast<uint4*>(sw + row * 128 + ((ch ^ (row & 7)) << 4)) = t[it];
   }
 }
 
@@ -244,7 +259,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8 * CL); }     // empty: one arrival per consumer warp of the cluster
+    // empty: one arrival per warp of the consuming warpgroup, in every CTA of the cluster
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4 * CL); }
     mbar_fence_init();
   }
   __syncthreads();
@@ -252,6 +268,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   if (warp < 4) {
     // ===================================================== TMA producer
+    setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int item = first_item; item < num_items; item += item_stride) {
@@ -289,14 +306,13 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   } else {
-    // ===================================================== consumers: wgmma main loop, then the epilogue
-    const int cwg = (warp >> 2) - 1;           // consumer warpgroup: accumulator rows 64 cwg .. + 63
-    const int ctid = threadIdx.x - 128;        // 0..255
-    const int e = warp - 4;                    // epilogue warp 0..7
-    const int quad = e & 3;                    // epilogue rows 32 quad .. + 31
-    const int part = e >> 2;                   // epilogue column slice
-    const int half = part;
-    uint8_t* sw = staging + e * Cfg::STG_WARP;
+    // ===================================================== consumers (ping-pong): wgmma main loop, then the epilogue
+    setmaxnreg_inc<232>();
+    // named barriers: 1 + cw accumulator tile written (this warpgroup), 3 + cw MMA turn of warpgroup cw, 5 + cw ACC turn of warpgroup cw
+    constexpr int BAR_TILE = 1, BAR_MMA = 3, BAR_ACC = 5;
+    const int cw = (warp >> 2) - 1;            // consumer warpgroup 0 / 1: items j = cw, cw + 2, .. of this CTA
+    const int quad = warp & 3;                 // epilogue rows 32 quad .. + 31; fragment rows 16 quad .. of each 64-row half
+    uint8_t* sw = staging + ((EPI == EPI_GEGLU ? 4 * cw : 0) + quad) * Cfg::STG_WARP;
     const int erow = quad * 32 + lane;         // this thread's accumulator row in the epilogue
     int stage = 0; uint32_t phase = 0;
     // a consumed ring slot is released in every CTA that wrote into it
@@ -307,30 +323,46 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         else mbar_arrive(&empty_bar[s]);
       }
     };
-    for (int item = first_item; item < num_items; item += item_stride) {
+    int nth = 0;                               // position of `item` in this CTA's sequence
+    for (int item = first_item; item < num_items; item += item_stride, ++nth) {
       const int split = item / unit_items;
       const int rem = item - split * unit_items;
       const int m_unit = rem / n_tiles, n_blk = rem - m_unit * n_tiles;
       const int m_blk = m_unit * CL + cta_rank;               // a tile past the end has rows_valid <= 0: every store below is row-guarded
       const int kb0 = split * kb_per_split;
       const int kb1 = min(kb0 + kb_per_split, kb_total);
-      float d[64];
+      if ((nth & 1) != cw) {                                 // the other warpgroup's item: step over its k-blocks in the ring
+        const int s = stage + (kb1 - kb0);
+        stage = s % STAGES;
+        phase ^= (uint32_t)(s / STAGES) & 1u;
+        continue;
+      }
+      // hand-offs pair up exactly: item nth waits for nth - 1's signal iff nth > 0, and signals iff there is an item nth + 1
+      const bool has_next = item + item_stride < num_items;
+      if (nth > 0) named_bar_sync(BAR_MMA + cw, 256);
+      float d0[64], d1[64];                                   // accumulator rows 0-63 / 64-127
 #pragma unroll
-      for (int i = 0; i < 64; ++i) d[i] = 0.f;
+      for (int i = 0; i < 64; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
       int prev_stage = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES);
         const uint32_t sB = sA + Cfg::A_BYTES;
-        wgmma_reg_fence(d);
+        wgmma_reg_fence(d0);
+        wgmma_reg_fence(d1);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < GEMM_BK / GEMM_UK; ++k) {
-          const uint64_t da = A_MN ? wgmma_desc_sw128(sA + cwg * (GEMM_BK * 128) + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
-                                   : wgmma_desc_sw128(sA + cwg * (64 * 128) + k * (GEMM_UK * 2), 16, 1024);
           const uint64_t db = B_MN ? wgmma_desc_sw128(sB + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
                                    : wgmma_desc_sw128(sB + k * (GEMM_UK * 2), 16, 1024);
-          wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, da, db, (kb > kb0 || k > 0) ? 1u : 0u);
+          // A rows 64-127: the second 64-wide MN block (MN-major) or 64 rows further down (K-major)
+          const uint64_t da0 = A_MN ? wgmma_desc_sw128(sA + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
+                                    : wgmma_desc_sw128(sA + k * (GEMM_UK * 2), 16, 1024);
+          const uint64_t da1 = A_MN ? wgmma_desc_sw128(sA + GEMM_BK * 128 + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
+                                    : wgmma_desc_sw128(sA + 64 * 128 + k * (GEMM_UK * 2), 16, 1024);
+          const uint32_t acc_flag = (kb > kb0 || k > 0) ? 1u : 0u;
+          wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d0, da0, db, acc_flag);
+          wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d1, da1, db, acc_flag);
         }
         wgmma_commit();
         wgmma_wait<1>();                        // the previous k-block's MMAs have retired: its smem slot is free
@@ -338,23 +370,26 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         prev_stage = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      if (has_next) named_bar_arrive(BAR_MMA + (cw ^ 1), 256);     // every k-block of this item is issued: the other main loop may start
       wgmma_wait<0>();
-      wgmma_reg_fence(d);
+      wgmma_reg_fence(d0);
+      wgmma_reg_fence(d1);
       if (prev_stage >= 0) release(prev_stage);
 
-      // ---- accumulator fragments -> shared fp32 tile (after every consumer has finished reading the previous tile's)
-      named_bar_sync(1, 256);
+      // ---- accumulator fragments -> shared fp32 tile, once the previous item's epilogue has finished reading it
+      if (nth > 0) named_bar_sync(BAR_ACC + cw, 256);
       {
-        const int w4 = (ctid >> 5) & 3;
-        const int r0 = cwg * 64 + w4 * 16 + (lane >> 2);
+        const int r0 = quad * 16 + (lane >> 2);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int c = 8 * j + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(acc + acc_off(r0, c)) = make_float2(d[4 * j], d[4 * j + 1]);
-          *reinterpret_cast<float2*>(acc + acc_off(r0 + 8, c)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+        for (int q = 0; q < 16; ++q) {
+          const int c = 8 * q + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(acc + acc_off(r0, c)) = make_float2(d0[4 * q], d0[4 * q + 1]);
+          *reinterpret_cast<float2*>(acc + acc_off(r0 + 8, c)) = make_float2(d0[4 * q + 2], d0[4 * q + 3]);
+          *reinterpret_cast<float2*>(acc + acc_off(r0 + 64, c)) = make_float2(d1[4 * q], d1[4 * q + 1]);
+          *reinterpret_cast<float2*>(acc + acc_off(r0 + 72, c)) = make_float2(d1[4 * q + 2], d1[4 * q + 3]);
         }
       }
-      named_bar_sync(1, 256);
+      named_bar_sync(BAR_TILE + cw, 128);
 
       const int wrow0 = m_blk * GEMM_BM + quad * 32;          // first row of this warp's 32-row slab
       const int row = wrow0 + lane;
@@ -369,7 +404,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const bool f32_staged = p.out_f32 && (p.row_off || (p.ld_f32 & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_f32) & 15) == 0);
         const bool bf16_staged = p.out_bf16 && (p.ld_bf16 & 7) == 0 && ((reinterpret_cast<uintptr_t>(p.out_bf16) & 15) == 0);
 #pragma unroll 1
-        for (int c = half * (BN / 64); c < (half + 1) * (BN / 64); ++c) {
+        for (int c = 0; c < BN / 32; ++c) {
           const int cbase = col0 + c * 32;
           if (cbase >= p.N) break;
           uint32_t r[32];
@@ -448,8 +483,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const float* gamma = kind == 0 ? p.q_gamma : p.k_gamma;
           __nv_bfloat16* dstm = kind == 0 ? p.q : p.k;
           const float2* cs = p.rope_cs + qk_pos;        // entry i of this row's position: cs[i * rope_len]
-          {
-            const int hh = half;
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {              // the tile's two heads
             uint32_t r0[32], r1[32];
             acc_ld32(acc, erow, hh * 64, r0);
             acc_ld32(acc, erow, hh * 64 + 32, r1);
@@ -481,8 +516,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             __syncwarp();
           }
         } else if (kind == 2) {
-          {
-            const int c = half;
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
             uint32_t r0[32], r1[32], w[32];
             acc_ld32(acc, erow, c * 64, r0);
             acc_ld32(acc, erow, c * 64 + 32, r1);
@@ -497,7 +532,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             else stg_store<8>(sw, lane, reinterpret_cast<uint8_t*>(p.v + (long long)wrow0 * HI + tis * 128 + c * 64), HI * 2, rows_valid);
             __syncwarp();
           }
-        } else if (half == 0) {
+        } else {
           uint32_t r[32];
           acc_ld32(acc, erow, 0, r);
           if (row_ok) {
@@ -515,12 +550,20 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const int crow = qk_pos;
         const float* zrow = (p.zgate && crow >= 0) ? p.zgate + (long long)crow * p.zgate_ld : nullptr;
         uint8_t* swb = sw + 4096;                       // 64-byte-pitch tile for the bf16 outputs
+        // the residual rows are requested one slice ahead: the global loads of slice sl + 1 are in flight while slice sl is computed
+        uint4 xres[8];
+        auto fetch = [&](int sl) {
+          stg_fetch(lane, reinterpret_cast<const uint8_t*>(p.x_res + (long long)wrow0 * p.N + col0 + sl * 32), (long long)p.N * 4,
+                    col0 + sl * 32 < p.N ? rows_valid : 0, xres);
+        };
+        fetch(0);
 #pragma unroll 1
-        for (int sl = part; sl < BN / 32; sl += 2) {    // 32-column slices of the tile
+        for (int sl = 0; sl < BN / 32; ++sl) {          // 32-column slices of the tile
           const int cbase = col0 + sl * 32;
           if (cbase >= p.N) break;                      // N is a multiple of 32 for every RESID use
           __syncwarp();
-          stg_load<8>(sw, lane, reinterpret_cast<const uint8_t*>(p.x_res + (long long)wrow0 * p.N + cbase), (long long)p.N * 4, rows_valid);
+          stg_fill(sw, lane, xres);
+          if (sl + 1 < BN / 32) fetch(sl + 1);
           uint32_t r[32];
           acc_ld32(acc, erow, sl * 32, r);
           float y[32];
@@ -580,32 +623,31 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           __syncwarp();
         }
       } else if constexpr (EPI == EPI_GEGLU) {
-        // the 128-wide tile is [64 value | 64 gate]; column slice `part` handles 32 value and the matching 32 gate columns
-        const int c = part;
-        const int cv = col0 + c * 32, cg = cv + 64;
-        if (cv < p.N) {                                 // N is a multiple of 128: a tile is either complete or absent
-          uint32_t r[32];
-          float g[32];
-          acc_ld32(acc, erow, c * 32, r);
-          {
-            float v[32];
+        // the 128-wide tile is [64 value | 64 gate]; column slice c handles 32 value and the matching 32 gate columns.  The whole
+        // accumulator row is read first and the tile handed on at once, so the GELU math and the stores overlap the next item's
+        // accumulator write (this warpgroup stages through its own four tiles).
+        uint32_t ra[4][32];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) + p.bias[cv + j];
-            stg64_put_pack(sw, lane, v);
-          }
+        for (int q = 0; q < 4; ++q) acc_ld32(acc, erow, q * 32, ra[q]);
+        if (has_next) named_bar_arrive(BAR_ACC + (cw ^ 1), 256);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int cv = col0 + c * 32, cg = cv + 64;
+          if (cv >= p.N) break;                         // N is a multiple of 128: a tile is either complete or absent
+          float v[32], g[32];                           // value and gate pre-activations stay in registers for the product
+#pragma unroll
+          for (int j = 0; j < 32; ++j) { v[j] = __uint_as_float(ra[c][j]) + p.bias[cv + j]; g[j] = __uint_as_float(ra[2 + c][j]) + p.bias[cg + j]; }
+          __syncwarp();
+          stg64_put_pack(sw, lane, v);
           __syncwarp();
           stg64_store(sw, lane, reinterpret_cast<uint8_t*>(p.vg + (long long)wrow0 * p.N + cv), (long long)p.N * 2, rows_valid);
-          acc_ld32(acc, erow, c * 32 + 64, r);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) g[j] = __uint_as_float(r[j]) + p.bias[cg + j];
           __syncwarp();
           stg64_put_pack(sw, lane, g);
           __syncwarp();
           stg64_store(sw, lane, reinterpret_cast<uint8_t*>(p.vg + (long long)wrow0 * p.N + cg), (long long)p.N * 2, rows_valid);
-          acc_ld32(acc, erow, c * 32, r);
 #pragma unroll
           for (int j = 0; j < 32; j += 2) {
-            const float2 o = geglu_pair(make_float2(g[j], g[j + 1]), make_float2(__uint_as_float(r[j]) + p.bias[cv + j], __uint_as_float(r[j + 1]) + p.bias[cv + j + 1]));
+            const float2 o = geglu_pair(make_float2(g[j], g[j + 1]), make_float2(v[j], v[j + 1]));
             g[j] = o.x; g[j + 1] = o.y;
           }
           __syncwarp();
@@ -615,6 +657,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           __syncwarp();
         }
       }
+      if (EPI != EPI_GEGLU && has_next) named_bar_arrive(BAR_ACC + (cw ^ 1), 256);   // accumulator and staging tiles are free for item nth + 1
     }
   }
   if constexpr (CL > 1) {

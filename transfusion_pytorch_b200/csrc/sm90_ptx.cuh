@@ -89,6 +89,16 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// signal a named barrier without waiting: the arriving threads count towards `count`, the waiting ones use named_bar_sync
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// ---------------------------------------------------------------- warpgroup register budget
+// Executed by every thread of a warpgroup: moves registers between the warpgroups of a CTA (the block's total stays what the
+// launch allocated, so the decreases must free what the increases take).
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ---------------------------------------------------------------- wgmma
 // A warpgroup (4 consecutive warps, the first a multiple of 4) issues each wgmma collectively.  Accumulator fragment of m64nN:
