@@ -63,6 +63,22 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
       ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_1d(const CUtensorMap* m, uint64_t* bar, void* smem, int c0) {
+  asm volatile(
+      "cp.async.bulk.tensor.1d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3}], [%2];"
+      ::"r"(smem_u32(smem)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0)
+      : "memory");
+}
+// global box (+)= shared tile, element-wise fp32 add in L2 (out-of-bounds box elements are skipped); completion by bulk group of the issuing thread
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, const void* smem, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem)), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// this thread's bulk groups have finished reading shared memory (the source tile may be rewritten)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// this thread's bulk groups are complete (writes performed)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // ---- clusters: a TMA load multicast into the same shared-memory offset of every CTA in `mask`; the completion bytes are counted on
 // the mbarrier at the same offset in each destination CTA
 __device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* m, uint64_t* bar, void* smem, int c0, int c1, uint16_t mask) {
