@@ -64,6 +64,11 @@ int tfx_gemm_resid(const void* A, long long lda, const void* A2, long long lda2,
 /* FeedForward net.0 + GEGLU (T.py:833-834, 846-847): W1 packed so every 128-column tile is [64 value | 64 gate];
  * writes the pre-activations vg [M][Np] (saved for backward) and h = gelu_erf(gate)*value [M][Np/2].           */
 int tfx_gemm_geglu(const void* u, long long ldu, const void* W1p, long long ldw, const float* b1p, int M, int Np, int K, void* vg, void* h, void* stream);
+/* the same with FeedForward dropout (T.py:845-850, nn.Dropout after GEGLU): h = gelu_erf(gate)*value * keep / (1 - p), vg undropped.
+ * keep is the counter-based mask of csrc/dropout.cuh (site 1: row = packed token, column = inner column, head 0), drawn from the
+ * device key drop_key (2 x u32, read at run time: a captured graph sees the key of each replay); p = 1 drops everything. */
+int tfx_gemm_geglu_drop(const void* u, long long ldu, const void* W1p, long long ldw, const float* b1p, int M, int Np, int K, void* vg, void* h,
+                        const void* drop_key /* device, 2 x u32 */, float p, int layer, void* stream);
 
 /* ---------------------------------------------------------------- attention (T.py:998-1027, mask T.py:452-470)
  * Flash-style, span mask from kv_limit[m] (last visible key of query m), tanh soft-cap, value gates in the epilogue.
@@ -174,6 +179,9 @@ int tfx_table_op(const float* a, long long ld_a, const float* b, long long ld_b,
  * updated with atomics directly. */
 int tfx_geglu_bwd_rows_per_block(void);
 int tfx_geglu_bwd(const void* dh_bf16, const void* vg_bf16, void* dvg_bf16, long long M, int inner_pad, const int* col_map, float* dbias, float* partials, void* stream);
+/* the same after tfx_gemm_geglu_drop: dh is multiplied by the regenerated mask and 1 / (1 - p) first */
+int tfx_geglu_bwd_drop(const void* dh_bf16, const void* vg_bf16, void* dvg_bf16, long long M, int inner_pad, const int* col_map, float* dbias, float* partials,
+                       const void* drop_key /* device, 2 x u32 */, float p, int layer, void* stream);
 /* text cross-entropy fwd+bwd (T.py:3320-3331; text-only 2653-2659 with vlimit = num_text_tokens) */
 int tfx_ce_fwd_bwd(const float* logits, long long ld_logits, const int* labels, int V, int vlimit, float gscale, void* dlogits_bf16, long long ld_dlogits,
                    double* loss_sum, int* n_valid, int M, void* stream);

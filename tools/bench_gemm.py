@@ -42,6 +42,7 @@ def main():
     cond_row = torch.randint(-1, n_cond, (M,), device = 'cuda', generator = g, dtype = torch.int32)
     zg = torch.rand(n_cond, 2 * D, device = 'cuda', generator = g)
     ls = torch.randn(D, device = 'cuda', generator = g) * 0.1
+    drop_key = torch.tensor([0x1234567, 0x7654321], device = 'cuda', dtype = torch.int32)      # FFN dropout p = 0.1 (csrc/dropout.cuh)
     cases = {   # name: (launch, algorithmic FLOPs, outputs to dump)
         'qkvg   [131072 x 1664 x 512]': (lambda: ops.gemm_qkvg(u, D, wq, D, M, H, D, q, k, v, gates, qk_inv, gq, gk, pos, rope_tt, 1024, None, None),
                                          2.0 * M * NQ * D, dict(q = q, k = k, v = v, gates = gates, qk_inv = qk_inv)),
@@ -50,6 +51,8 @@ def main():
         'resid  [131072 x 512 x 1408]': (lambda: ops.gemm_resid(h, Ip, None, 0, 0, w2r, Ip, M, D, Ip, bias2, x_b, None, x_cb, yF, cond_row, zg[:, :D], 2 * D, ls),
                                          2.0 * M * D * Ip, dict(x_out_bf16 = x_cb, y = yF)),
         'geglu  [131072 x 2816 x 512]': (lambda: ops.gemm_geglu(u, D, w1, D, b1, M, 2 * Ip, D, vg, h), 2.0 * M * 2 * Ip * D, dict(vg = vg, h = h)),
+        'geglu_drop [131072 x 2816 x 512]': (lambda: ops.gemm_geglu_drop(u, D, w1, D, b1, M, 2 * Ip, D, vg, h, drop_key, 0.1, 0), 2.0 * M * 2 * Ip * D,
+                                             dict(vg = vg, h = h)),
         'store  [131072 x 2816 x 512]': (lambda: ops.gemm_store(u, D, 0, w1, D, 0, M, 2 * Ip, D, None, 0, vg, 2 * Ip, None, None, 1.0, 0, 1), 2.0 * M * 2 * Ip * D,
                                          dict(out = vg)),
         'dgrad  [131072 x 1408 x 512]': (lambda: ops.gemm_store(dy, D, 0, w2, Ip, 1, M, Ip, D, None, 0, dh, Ip, None, None, 1.0, 0, 1), 2.0 * M * Ip * D, dict(out = dh)),

@@ -24,6 +24,7 @@ SIGNATURES = {
     'tfx_gemm_qkvg': [VP, LL, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP],
     'tfx_gemm_resid': [VP, LL, VP, LL, I, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, VP, LL, VP, VP],
     'tfx_gemm_geglu': [VP, LL, VP, LL, VP, I, I, I, VP, VP, VP],
+    'tfx_gemm_geglu_drop': [VP, LL, VP, LL, VP, I, I, I, VP, VP, VP, F, I, VP],
     'tfx_attn_fwd': [VP, VP, VP, LL, LL, LL, VP, I, VP, VP, VP, VP, VP, I, VP, LL, VP, I, F, F, VP, VP],
     'tfx_attn_fwd_tc': [VP, VP, VP, LL, LL, LL, VP, I, VP, VP, VP, VP, VP, I, VP, LL, VP, I, I, F, F, VP, VP],
     'tfx_attn_fast_params': [VP, VP, I, F, F, VP, VP],
@@ -48,6 +49,7 @@ SIGNATURES = {
     'tfx_time_features': [VP, VP, VP, I, I, I, VP],
     'tfx_table_op': [VP, LL, VP, LL, VP, LL, VP, LL, LL, I, I, VP],
     'tfx_geglu_bwd': [VP, VP, VP, LL, I, VP, VP, VP, VP],
+    'tfx_geglu_bwd_drop': [VP, VP, VP, LL, I, VP, VP, VP, VP, F, I, VP],
     'tfx_ce_fwd_bwd': [VP, LL, VP, I, I, F, VP, LL, VP, VP, I, VP],
     'tfx_mse_fwd_bwd': [VP, LL, VP, VP, LL, F, VP, LL, I, VP],
     'tfx_colsum_bf16': [VP, LL, LL, I, VP, VP, VP],

@@ -88,4 +88,16 @@ int tfx_gemm_geglu(const void* u, long long ldu, const void* W1p, long long ldw,
   return finish(launch_gemm_t<false, false, EPI_GEGLU>(a, b, p, num_sms(), ST(stream)), "gemm_geglu");
 }
 
+int tfx_gemm_geglu_drop(const void* u, long long ldu, const void* W1p, long long ldw, const float* b1p, int M, int Np, int K, void* vg, void* h,
+                        const void* drop_key, float p_drop, int layer, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(Np % 128 == 0, "gemm_geglu_drop: packed N (%d) must be a multiple of 128", Np);
+  TFX_REQUIRE(drop_key && p_drop >= 0.f && p_drop <= 1.f && layer >= 0, "gemm_geglu_drop: needs a device key, p in [0, 1] (got %g) and layer >= 0 (got %d)", (double)p_drop, layer);
+  GemmParams p; memset(&p, 0, sizeof(p));
+  p.M = M; p.N = Np; p.K = K; p.k_splits = 1; p.bias = b1p; p.vg = (__nv_bfloat16*)vg; p.h = (__nv_bfloat16*)h;
+  p.drop = make_drop_params(drop_key, p_drop, layer);
+  GemmOperand a{u, ldu, false}, b{W1p, ldw, false};
+  return finish(launch_gemm_t<false, false, EPI_GEGLU_DROP>(a, b, p, num_sms(), ST(stream)), "gemm_geglu_drop");
+}
+
 }  // extern "C"

@@ -30,6 +30,7 @@
 // A ring slot is refilled only after the consumers of BOTH CTAs have released it (they arrive on the empty barriers of both).
 #pragma once
 #include "sm90_ptx.cuh"
+#include "dropout.cuh"
 
 namespace tfx {
 
@@ -38,7 +39,7 @@ constexpr int GEMM_BN = 128;
 constexpr int GEMM_BK = 64;     // 64 bf16 = 128 B = one swizzle atom row
 constexpr int GEMM_UK = 16;     // wgmma K for 16-bit inputs
 
-enum : int { EPI_STORE = 0, EPI_QKVG = 1, EPI_RESID = 2, EPI_GEGLU = 3 };
+enum : int { EPI_STORE = 0, EPI_QKVG = 1, EPI_RESID = 2, EPI_GEGLU = 3, EPI_GEGLU_DROP = 4 };   // GEGLU_DROP: GEGLU with FFN dropout on h
 
 struct GemmParams {
   int M, N, K;                 // D is M x N, reduction K
@@ -72,7 +73,8 @@ struct GemmParams {
   const float* ls;             // [N] layerscale (scale = ls + 1 for text rows); null => scale = 1
   // ---- EPI_GEGLU (N tile 128 = [64 value cols | 64 gate cols], N = 2*inner_pad)
   __nv_bfloat16* vg;           // [M][N] pre-activation (value|gate interleaved per tile), saved for backward
-  __nv_bfloat16* h;            // [M][N/2] gelu(gate)*value
+  __nv_bfloat16* h;            // [M][N/2] gelu(gate)*value (EPI_GEGLU_DROP: times mask / (1 - p); vg stays undropped)
+  DropParams drop;             // EPI_GEGLU_DROP only (dropout.cuh, site FFN: i = row, j = column of h)
 };
 
 template <int EPI> struct GemmCfg {
@@ -85,7 +87,7 @@ template <int EPI> struct GemmCfg {
   // per-warp staging: 32 rows x 128 B; RESID adds a 64-byte-pitch bf16 tile (2 KB).  Four warps (one epilogue warpgroup at a
   // time), except GEGLU: its warpgroups hand the accumulator tile over before their epilogues end, so each has its own four.
   static constexpr int STG_WARP = EPI == 2 ? 4096 + 2048 : 4096;
-  static constexpr int STAGING = (EPI == 3 ? 8 : 4) * STG_WARP;
+  static constexpr int STAGING = (EPI >= 3 ? 8 : 4) * STG_WARP;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + STAGING + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one block");
 };
@@ -232,6 +234,7 @@ template <bool A_MN, bool B_MN, int EPI, int CL>
 __global__ void __launch_bounds__(384, 1)
 gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using Cfg = GemmCfg<EPI>;
+  constexpr bool GEGLU = EPI == EPI_GEGLU || EPI == EPI_GEGLU_DROP;
   constexpr int BN = GEMM_BN;
   constexpr int STAGES = Cfg::STAGES;
   static_assert(Cfg::STAGE_BYTES % 1024 == 0 && 2 * STAGES <= 32, "stage alignment / barrier area");
@@ -312,7 +315,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     constexpr int BAR_TILE = 1, BAR_MMA = 3, BAR_ACC = 5;
     const int cw = (warp >> 2) - 1;            // consumer warpgroup 0 / 1: items j = cw, cw + 2, .. of this CTA
     const int quad = warp & 3;                 // epilogue rows 32 quad .. + 31; fragment rows 16 quad .. of each 64-row half
-    uint8_t* sw = staging + ((EPI == EPI_GEGLU ? 4 * cw : 0) + quad) * Cfg::STG_WARP;
+    uint8_t* sw = staging + ((GEGLU ? 4 * cw : 0) + quad) * Cfg::STG_WARP;
     const int erow = quad * 32 + lane;         // this thread's accumulator row in the epilogue
     int stage = 0; uint32_t phase = 0;
     // a consumed ring slot is released in every CTA that wrote into it
@@ -622,10 +625,18 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
           __syncwarp();
         }
-      } else if constexpr (EPI == EPI_GEGLU) {
+      } else if constexpr (GEGLU) {
         // the 128-wide tile is [64 value | 64 gate]; column slice c handles 32 value and the matching 32 gate columns.  The whole
         // accumulator row is read first and the tile handed on at once, so the GELU math and the stores overlap the next item's
         // accumulator write (this warpgroup stages through its own four tiles).
+        // dropout: the keep bits of the row's 64 h columns (one Philox call per 8), computed before the accumulator row is loaded,
+        // where few registers are live (drawn later, next to the 128 accumulator words, they spill)
+        uint32_t keep[2] = {0u, 0u};
+        if constexpr (EPI == EPI_GEGLU_DROP) {
+          const uint32_t k0 = __ldg(p.drop.key), k1 = __ldg(p.drop.key + 1);
+#pragma unroll
+          for (int q = 0; q < 8; ++q) keep[q >> 2] |= drop_keep8(p.drop, k0, k1, DROP_SITE_FFN, 0, (uint32_t)row, (uint32_t)(n_blk * 8 + q)) << (8 * (q & 3));
+        }
         uint32_t ra[4][32];
 #pragma unroll
         for (int q = 0; q < 4; ++q) acc_ld32(acc, erow, q * 32, ra[q]);
@@ -650,6 +661,10 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             const float2 o = geglu_pair(make_float2(g[j], g[j + 1]), make_float2(v[j], v[j + 1]));
             g[j] = o.x; g[j + 1] = o.y;
           }
+          if constexpr (EPI == EPI_GEGLU_DROP) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) g[j] = (keep[c] >> j) & 1u ? g[j] * p.drop.scale : 0.f;
+          }
           __syncwarp();
           stg64_put_pack(sw, lane, g);
           __syncwarp();
@@ -657,7 +672,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           __syncwarp();
         }
       }
-      if (EPI != EPI_GEGLU && has_next) named_bar_arrive(BAR_ACC + (cw ^ 1), 256);   // accumulator and staging tiles are free for item nth + 1
+      if (!GEGLU && has_next) named_bar_arrive(BAR_ACC + (cw ^ 1), 256);   // accumulator and staging tiles are free for item nth + 1
     }
   }
   if constexpr (CL > 1) {

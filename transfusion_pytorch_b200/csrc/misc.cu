@@ -4,6 +4,7 @@
 // Reference math: modality_processing.py:645-656 (noise), transfusion.py:617-635 (fourier), 831-834
 // (GEGLU), 3320-3376 (loss heads).
 #include "common.cuh"
+#include "dropout.cuh"
 #include "../../include/tfx_b200.h"
 #include <math.h>
 
@@ -86,8 +87,11 @@ __global__ void table_op_k(const float* __restrict__ a, const float* __restrict_
 // GEGLU backward on the tile-interleaved layout ([64 value | 64 gate] per 128 columns), fused with the column sums of
 // d(vg) (= gradient of the FFN-in bias).  A thread owns one 8-column chunk of h (and the matching value / gate chunks)
 // and walks `rpb` rows; its 16 column sums stay in registers and are flushed with one atomicAdd each per block.
-__global__ void geglu_bwd_k(const __nv_bfloat16* __restrict__ dh, const __nv_bfloat16* __restrict__ vg, __nv_bfloat16* __restrict__ dvg, long long M, int Ip,
-                            const int* __restrict__ col_map, float* __restrict__ dbias, float* __restrict__ partials, int rpb) {
+// DROP: h was dropped in the forward (site FFN), so dh is first multiplied by the regenerated mask and 1 / (1 - p).
+template <bool DROP>
+__device__ __forceinline__ void geglu_bwd_body(const __nv_bfloat16* __restrict__ dh, const __nv_bfloat16* __restrict__ vg, __nv_bfloat16* __restrict__ dvg, long long M,
+                                               int Ip, const int* __restrict__ col_map, float* __restrict__ dbias, float* __restrict__ partials, int rpb,
+                                               const DropParams& drop) {
   const int cpr = Ip / 8;                 // 16-byte chunks per row of dh
   const int ch = threadIdx.x;
   if (ch >= cpr) return;
@@ -105,9 +109,16 @@ __global__ void geglu_bwd_k(const __nv_bfloat16* __restrict__ dh, const __nv_bfl
     const uint4 g4 = *reinterpret_cast<const uint4*>(vrow + 64 + j);
     const uint32_t dw[4] = {d4.x, d4.y, d4.z, d4.w}, vw[4] = {v4.x, v4.y, v4.z, v4.w}, gw[4] = {g4.x, g4.y, g4.z, g4.w};
     uint32_t ov[4], og[4];
+    uint32_t keep = 0;
+    if constexpr (DROP) keep = drop_keep8(drop, __ldg(drop.key), __ldg(drop.key + 1), DROP_SITE_FFN, 0, (uint32_t)r, (uint32_t)ch);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float2 d = unpack2_bf16(dw[k]), v = unpack2_bf16(vw[k]), g = unpack2_bf16(gw[k]);
+      float2 d = unpack2_bf16(dw[k]);
+      const float2 v = unpack2_bf16(vw[k]), g = unpack2_bf16(gw[k]);
+      if constexpr (DROP) {
+        d.x = (keep >> (2 * k)) & 1u ? d.x * drop.scale : 0.f;
+        d.y = (keep >> (2 * k + 1)) & 1u ? d.y * drop.scale : 0.f;
+      }
       float cdf0, pdf0, cdf1, pdf1;
       gelu_parts(g.x, cdf0, pdf0); gelu_parts(g.y, cdf1, pdf1);
       const float ov0 = d.x * g.x * cdf0, ov1 = d.y * g.y * cdf1;                       // d value = dh * gelu(g)
@@ -135,6 +146,15 @@ __global__ void geglu_bwd_k(const __nv_bfloat16* __restrict__ dh, const __nv_bfl
       if (og_ >= 0) atomicAdd(dbias + og_, sg[e]);
     }
   }
+}
+
+__global__ void geglu_bwd_k(const __nv_bfloat16* __restrict__ dh, const __nv_bfloat16* __restrict__ vg, __nv_bfloat16* __restrict__ dvg, long long M, int Ip,
+                            const int* __restrict__ col_map, float* __restrict__ dbias, float* __restrict__ partials, int rpb) {
+  geglu_bwd_body<false>(dh, vg, dvg, M, Ip, col_map, dbias, partials, rpb, DropParams{});
+}
+__global__ void geglu_bwd_drop_k(const __nv_bfloat16* __restrict__ dh, const __nv_bfloat16* __restrict__ vg, __nv_bfloat16* __restrict__ dvg, long long M, int Ip,
+                                 const int* __restrict__ col_map, float* __restrict__ dbias, float* __restrict__ partials, int rpb, const DropParams drop) {
+  geglu_bwd_body<true>(dh, vg, dvg, M, Ip, col_map, dbias, partials, rpb, drop);
 }
 
 // text cross-entropy, forward + backward in one pass (one warp per token)
@@ -397,6 +417,18 @@ int tfx_geglu_bwd(const void* dh_bf16, const void* vg_bf16, void* dvg_bf16, long
   geglu_bwd_k<<<(unsigned)((M + rpb - 1) / rpb), threads, 0, ST(stream)>>>((const __nv_bfloat16*)dh_bf16, (const __nv_bfloat16*)vg_bf16, (__nv_bfloat16*)dvg_bf16, M, inner_pad,
                                                                          col_map, dbias, partials, rpb);
   return check_launch("geglu_bwd");
+}
+
+int tfx_geglu_bwd_drop(const void* dh_bf16, const void* vg_bf16, void* dvg_bf16, long long M, int inner_pad, const int* col_map, float* dbias, float* partials,
+                       const void* drop_key, float p_drop, int layer, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(inner_pad % 64 == 0 && inner_pad <= 8192, "geglu_bwd_drop: inner_pad %d must be a multiple of 64 and <= 8192", inner_pad);
+  TFX_REQUIRE(drop_key && p_drop >= 0.f && p_drop <= 1.f && layer >= 0, "geglu_bwd_drop: needs a device key, p in [0, 1] (got %g) and layer >= 0 (got %d)", (double)p_drop, layer);
+  const int threads = ((inner_pad / 8) + 31) / 32 * 32;
+  const int rpb = tfx_geglu_bwd_rows_per_block();
+  geglu_bwd_drop_k<<<(unsigned)((M + rpb - 1) / rpb), threads, 0, ST(stream)>>>((const __nv_bfloat16*)dh_bf16, (const __nv_bfloat16*)vg_bf16, (__nv_bfloat16*)dvg_bf16, M,
+                                                                              inner_pad, col_map, dbias, partials, rpb, make_drop_params(drop_key, p_drop, layer));
+  return check_launch("geglu_bwd_drop");
 }
 
 int tfx_ce_fwd_bwd(const float* logits, long long ld_logits, const int* labels, int V, int vlimit, float gscale, void* dlogits_bf16, long long ld_dlogits,

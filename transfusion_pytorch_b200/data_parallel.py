@@ -90,11 +90,12 @@ class DataParallelTrainer:
         return (rb.M, rb.B, rb.n_cond, rb.S, tuple(rb.type_rows), tuple(getattr(rb, n).shape[0] if getattr(rb, n) is not None else 0 for n in eng.META_NAMES), rb.total_tokens,
                 tuple(rb.n_type_tokens), (rb.max_rope_pos + 1 + 1023) // 1024, rb.has_labels, rb.pos_max)
 
-    def _graph_step(self, rb, device_lat = None, noise = None):
+    def _graph_step(self, rb, device_lat = None, noise = None, dropout_key = None):
         """Returns the loss of a replayed (or freshly captured) step, or None when this batch must run eagerly.
         device_lat: per-type latent matrices already on the device (then rb must be uploaded too: a device-resident batch)."""
         model, eng = self.model, self.model.engine
-        sig = self._signature(rb, eng)
+        drop = model.transformer.ff_dropout_p(True, model.training) > 0.
+        sig = self._signature(rb, eng) + (drop,)          # a step with dropout launches other kernels than one without
         g = self._graphs.get(sig)
         if g is None:
             if len(self._graphs) >= 8:
@@ -117,6 +118,7 @@ class DataParallelTrainer:
             g.lat = [torch.empty(s1 - s0, model.dim_latents[t], device = eng.device, dtype = torch.float32) if s1 > s0 else None for t, (s0, s1) in enumerate(rb.type_rows)]
             g.lat_stage = [torch.empty_like(l) if l is not None else None for l in g.lat]
             g.eps = [torch.empty_like(l) if l is not None else None for l in g.lat]      # flow noise: a static input of the graph, drawn (or injected) per step
+            g.drop_key = torch.zeros(2, device = eng.device, dtype = torch.int32)     # dropout key: likewise
             g.consumed = torch.cuda.Event()
             g.consumed.record()
         assert layout == g.layout
@@ -150,6 +152,8 @@ class DataParallelTrainer:
                     e.copy_(noise[t].reshape(e.shape), non_blocking = True)      # injected (deterministic parity runs)
                 else:
                     e.normal_()
+        if drop:
+            eng.dropout_key(dropout_key, out = g.drop_key)
         if getattr(eng, 'opt_step_dev', None) is None:
             eng.opt_step_dev = torch.zeros(1, device = eng.device, dtype = torch.int32)
         eng.opt_step_dev.fill_(eng.opt_step)             # device-resident optimizer step counter (incremented inside the graph)
@@ -167,7 +171,8 @@ class DataParallelTrainer:
             graph = torch.cuda.CUDAGraph()
             l0 = eng.ops.launches
             with torch.cuda.graph(graph):
-                res = eng.forward(rb, g.lat, g.eps, train = True, text_loss_weight = model.text_loss_weight, flow_loss_weight = model.flow_loss_weight)
+                res = eng.forward(rb, g.lat, g.eps, train = True, text_loss_weight = model.text_loss_weight, flow_loss_weight = model.flow_loss_weight,
+                                  dropout = model.training, dropout_key = g.drop_key)
                 # NCCL all-reduce of the flat gradient buffer captured INSIDE the step graph: per-layer buckets on the communication stream, forked
                 # from / joined to the capture stream, so the collective of layers >= i overlaps the backward kernels of layers < i on every replay
                 self._backward_allreduce(eng, lambda cb: eng.backward(bucket_cb = cb))
@@ -246,14 +251,14 @@ class DataParallelTrainer:
             if self.world > 1:
                 dist.all_reduce(eng.gflat)
 
-    def step_packed_eager(self, rb, latents, noise = None):
+    def step_packed_eager(self, rb, latents, noise = None, dropout_key = None):
         """the step of `step_packed` launched eagerly (profiling passes, shapes that are not captured)"""
         model, eng = self.model, self.model.engine
         eng.ensure_attached()
         self._sync_replicas(eng)
         eng.upload(rb)
         eng.zero_grad()
-        loss = model.forward_packed(rb, latents, noise = noise)
+        loss = model.forward_packed(rb, latents, noise = noise, dropout_key = dropout_key)
         def run(cb):
             eng._bucket_cb = cb
             loss.backward()
@@ -270,16 +275,17 @@ class DataParallelTrainer:
         if self.ema_decay is not None:
             eng.ema_update(self.ema_decay)
 
-    def step_packed(self, rb, latents, noise = None):
+    def step_packed(self, rb, latents, noise = None, dropout_key = None):
         """One training step from a packed batch that is already resident on the device (`model.pack` + `engine.upload` + latents on the
-        device): CUDA-graph replay when the shape signature has been seen before, eager launches otherwise.  Single process only."""
+        device): CUDA-graph replay when the shape signature has been seen before, eager launches otherwise.  Single process only.
+        `noise` / `dropout_key` (optional): injected flow noise and dropout key (`Transfusion.forward`) for deterministic runs."""
         model, eng = self.model, self.model.engine
         eng.ensure_attached()
         self._sync_replicas(eng)
         eng.upload(rb)
-        loss = self._graph_step(rb, device_lat = latents, noise = noise) if self.cuda_graph else None
+        loss = self._graph_step(rb, device_lat = latents, noise = noise, dropout_key = dropout_key) if self.cuda_graph else None
         if loss is None:
-            loss = self.step_packed_eager(rb, latents, noise = noise)
+            loss = self.step_packed_eager(rb, latents, noise = noise, dropout_key = dropout_key)
         return loss
 
     def step(self, batch, times = None, noise = None, **fw):

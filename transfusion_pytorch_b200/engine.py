@@ -401,16 +401,19 @@ class Engine:
     # ------------------------------------------------------------------ forward
     def forward(self, rb: RaggedBatch, latents: list | None, eps: list | None, *, train: bool, want_logits = False, vlimit = 0,
                 text_loss_weight = 1., flow_loss_weight = 1., modality_only = False, cache: KVCache | None = None, want_preds = None,
-                vel_targets = None, vel_weight = 0.):
+                vel_targets = None, vel_weight = 0., dropout = False, dropout_key = None):
         """Runs the block stack over a ragged batch.  `latents[t]`: fp32 [S_t, dl_t] device tensors (clean latents when
         `eps` is given, already-noised / decode-time latents otherwise).  With train=True activations are kept for
-        `backward()` and the fused loss heads produce the loss scalars and the head gradients in the same pass."""
+        `backward()` and the fused loss heads produce the loss scalars and the head gradients in the same pass.
+        `dropout`: the owning module is in training mode; FFN dropout then applies to a train forward (`Transformer.ff_dropout_p`), with the
+        masks of `dropout_key` (see `dropout_key()`)."""
         self.ensure_attached()
         self.pack_weights(force = train)
         o, D, HI, H, Ip, M = self.ops, self.D, self.HI, self.H, self.Ip, rb.M
         dv = self.upload(rb)
         nc, S = rb.n_cond, rb.S
-        st = self.state = dict(rb = rb, train = train, layers = [])
+        p_ff = self.model.transformer.ff_dropout_p(train, dropout)
+        st = self.state = dict(rb = rb, train = train, layers = [], p_ff = p_ff, drop_key = self.dropout_key(dropout_key) if p_ff > 0. else None)
         pk = self.packed
         rope = self.rope_table(rb.max_rope_pos)
         cond_row = dv['cond_row'] if nc > 0 else None
@@ -542,7 +545,10 @@ class Engine:
             uF = self.buf(f'{lt}uF', (M, D), BF16); statsF = self.buf(f'{lt}sF', (M, 2), F32)
             o.adaln_fwd(x_b, cond_row, filmF, tab_ld, self.P(f'{pre}.2.layernorm_gamma'), uF, statsF, M, D)
             vg = self.buf(f'{lt}vg', (M, 2 * Ip), BF16); h = self.buf(f'{lt}h', (M, Ip), BF16)
-            o.gemm_geglu(uF, D, pk[f'w1{i}'], D, pk[f'b1{i}'], M, 2 * Ip, D, vg, h)
+            if p_ff > 0.:
+                o.gemm_geglu_drop(uF, D, pk[f'w1{i}'], D, pk[f'b1{i}'], M, 2 * Ip, D, vg, h, st['drop_key'], p_ff, i)
+            else:
+                o.gemm_geglu(uF, D, pk[f'w1{i}'], D, pk[f'b1{i}'], M, 2 * Ip, D, vg, h)
             yF = self.buf(f'{lt}yF', (M, D), BF16) if train else None
             if self.hid_bf16:                                # x_c feeds nothing but the AttentionResiduals: keep the bf16 copy only
                 x_c = self.buf(f'{tag}Hb{i + 1}', (M, D), BF16)
@@ -659,6 +665,20 @@ class Engine:
             vel = [vel_terms.get(t, torch.zeros((), device = self.device)) for t in range(len(self.dls))] if vel_terms else None
             res.update(loss_acc = acc, n_valid = nvalid, total = total, text = text, flows = flows, vel = vel)
         return res
+
+    def dropout_key(self, src = None, out: Tensor | None = None) -> Tensor:
+        """Device key (int32 [2] holding the two u32 words) of a forward's dropout masks (csrc/dropout.cuh).  `src` None: drawn from torch's
+        CUDA generator, so `torch.manual_seed` reproduces a run; (k0, k1): those words (deterministic runs); a device int32 [2] tensor: used
+        as is.  `out`: the int32 [2] device tensor to fill instead of the engine's own (a captured step graph's static input)."""
+        if torch.is_tensor(src):
+            assert src.dtype == I32 and src.numel() == 2 and src.device == self.device, 'a dropout key tensor is int32 [2] on the engine device'
+            return src
+        key = out if out is not None else self.buf('drop_key', (2,), I32)
+        if src is None:
+            key.random_(-2 ** 31, 2 ** 31)
+        else:
+            key.copy_(torch.from_numpy(np.array(src, dtype = np.uint32).view(np.int32)))
+        return key
 
     def _prepare_grads(self):
         """`.grad` of every trainable parameter must be its view of the flat gradient buffer (kernels accumulate there)."""
@@ -786,7 +806,10 @@ class Engine:
             rpb = self.ops.lib.tfx_geglu_bwd_rows_per_block()
             nblk = (M + rpb - 1) // rpb
             part = self.buf('geglu_part', (nblk, 2 * Ip), F32)
-            o.geglu_bwd(dh, L['vg'], dvg, M, Ip, None, None, part)
+            if st['p_ff'] > 0.:
+                o.geglu_bwd_drop(dh, L['vg'], dvg, M, Ip, None, None, part, st['drop_key'], st['p_ff'], i)
+            else:
+                o.geglu_bwd(dh, L['vg'], dvg, M, Ip, None, None, part)
             o.colsum_f32(part, 2 * Ip, nblk, 2 * Ip, lm['b1_cols'], self.gflat)
             o.gemm_store(dvg, 2 * Ip, 0, pk[f'w1{i}'], D, 1, M, D, 2 * Ip, du, D, None, 0, None, None, 1.0, 0, 1)
             o.gemm_store(dvg, 2 * Ip, 1, L['uF'], D, 1, 2 * Ip, D, M, self.gflat, 0, None, 0, None, lm['w1_rows'], 1.0, 1, ksplit(2 * Ip, D))

@@ -94,6 +94,15 @@ def small_batch(batch: int, seed: int = 0, **kw):
     return [small_sample(seed * 7919 + b, **kw) for b in range(batch)]
 
 
+def dropout_batch(dim_latent: int = 32, text_vocab: int = 64, seed: int = 11):
+    """Three interleaved samples, text | modality | text | modality | text, of odd packed lengths (37, 43 and 45 tokens with [sos] / [eos]
+    and the modality delimiters): the FFN-dropout fixture, tests/golden/small_dropout.pt."""
+    g = _gen(seed)
+    shapes = [(5, 7, 4, 9, 3), (8, 12, 1, 6, 6), (2, 5, 11, 13, 4)]       # text, latents, text, latents, text
+    return [[torch.randint(0, text_vocab, (n,), generator = g) if k % 2 == 0 else torch.randn(n, dim_latent, generator = g) for k, n in enumerate(s)]
+            for s in shapes]
+
+
 def config4_sample(seed: int, total_len: int = 1025, dims = (384, 192), text_vocab: int = 256):
     """Two modality types, many short alternating spans (span-mask stress), padded with text so that the
     packed length is exactly `total_len` after [sos]/[eos] and meta tokens."""

@@ -203,12 +203,19 @@ class Transformer(Module):
         super().__init__()
         unsupported = []
         if dim_head != 64: unsupported.append('dim_head != 64')
-        if dropout != 0.: unsupported.append('dropout > 0')
+        ff_dropout = float(ff_kwargs.get('dropout', 0.))
+        for name, p in (('dropout', dropout), ("ff_kwargs['dropout']", ff_dropout)):
+            if not 0. <= p <= 1.:
+                raise ValueError(f'{name} probability has to be between 0 and 1, but got {p}')      # nn.Dropout's check
+        # attention dropout (T.py:1017) is not implemented by the attention kernels.  With use_flex_attn the reference takes the flex_attention
+        # branch on CUDA (T.py:987-995), which applies no attention dropout, so there `dropout` is accepted and has no effect.
+        if dropout != 0. and not use_flex_attn: unsupported.append('dropout > 0 (attention dropout) without use_flex_attn')
         if use_value_residual and heads > 16: unsupported.append('use_value_residual with heads > 16')
         if not qk_rmsnorm: unsupported.append('qk_rmsnorm = False')
         extra = set(attn_kwargs) - {'softcap_value', 'laser_softclamp_value'}
         if extra: unsupported.append(f'attn_kwargs {sorted(extra)}')
-        if ff_kwargs: unsupported.append(f'ff_kwargs {sorted(ff_kwargs)}')
+        extra = set(ff_kwargs) - {'dropout'}         # FeedForward(dim, mult, dropout) (T.py:837-850): dropout is its only option besides the two above
+        if extra: unsupported.append(f'ff_kwargs {sorted(extra)}')
         if unsupported:
             raise NotImplementedError('not implemented by the CUDA kernels: ' + ', '.join(unsupported))
         self.dim, self.depth, self.dim_head, self.heads = dim, depth, dim_head, heads
@@ -218,6 +225,7 @@ class Transformer(Module):
         self.laser_softclamp_value = float(attn_kwargs.get('laser_softclamp_value', 15.))
         self.softcap_value = float(attn_kwargs.get('softcap_value', 50.))
         self.ff_inner = int(dim * ff_expansion_factor * 2 / 3)
+        self.ff_dropout = ff_dropout                 # nn.Dropout after GEGLU (T.py:848): fused into the GEGLU GEMM epilogue, training forwards only
 
         self.to_time_cond = nn.Sequential(_Fourier(dim), nn.Linear(dim + 1, dim * 4), nn.SiLU())
         layers = ModuleList([])
@@ -228,6 +236,11 @@ class Transformer(Module):
             layers.append(ModuleList([skip_proj, attn, ff, _AttnResidualParams(dim)]))
         self.layers = layers
         self.norm = _Gamma(dim)
+
+    def ff_dropout_p(self, train: bool, training: bool) -> float:
+        """FFN dropout probability of one forward: nn.Dropout drops only in training mode (`training`, of the owning Transfusion), and only a
+        forward that keeps its activations for a backward (`train`) is a training forward; sampling, eval and the EMA teacher never drop."""
+        return self.ff_dropout if (train and training) else 0.
 
     def forward(self, *args, **kwargs):
         raise RuntimeError('Transformer.forward is executed by the CUDA engine through Transfusion; call the Transfusion methods')
@@ -465,33 +478,35 @@ class Transfusion(SamplingMixin, Module):
                 POOL.give(stage_raw)
         return nbytes
 
-    def _run(self, rb, latents, eps, *, train, **kw):
+    def _run(self, rb, latents, eps, *, train, dropout_key = None, **kw):
         eng = self.engine
+        if self.transformer.ff_dropout_p(train, self.training) > 0.:
+            kw.update(dropout = True, dropout_key = dropout_key)
         if train and torch.is_grad_enabled():
             anchor = self.text_embed.weight
             total, text, flows = _TrainStep.apply(eng, rb, latents, eps, kw, anchor)
             return dict(total = total, text = text, flows = flows, vel = eng._last_vel)
         return eng.forward(rb, latents, eps, train = train, **kw)
 
-    def forward_packed(self, rb: RaggedBatch, latents: list, noise: list | None = None, return_breakdown = False):
+    def forward_packed(self, rb: RaggedBatch, latents: list, noise: list | None = None, return_breakdown = False, dropout_key = None):
         """Training step from an already packed (and possibly already uploaded) ragged batch: the part of `forward`
-        after pack/route.  Used by bench.py to time the device-resident path."""
+        after pack/route.  Used by bench.py to time the device-resident path.  `dropout_key`: see `forward`."""
         eps = noise if exists(noise) else [torch.randn_like(l) if exists(l) else None for l in latents]
-        res = self._run(rb, latents, eps, train = True, text_loss_weight = self.text_loss_weight, flow_loss_weight = self.flow_loss_weight)
+        res = self._run(rb, latents, eps, train = True, text_loss_weight = self.text_loss_weight, flow_loss_weight = self.flow_loss_weight, dropout_key = dropout_key)
         self._last_batch = rb
         if return_breakdown:
             return res['total'], LossBreakdown(res['total'], res['text'], list(res['flows']), None, None)
         return res['total']
 
     # ------------------------------------------------------------------ text only (transfusion.py:2585-2707)
-    def forward_text(self, text: Tensor, return_loss = True, return_embed = False, cache = None, return_hiddens = False, return_kv_cache = False):
+    def forward_text(self, text: Tensor, return_loss = True, return_embed = False, cache = None, return_hiddens = False, return_kv_cache = False, dropout_key = None):
         """`cache` / `return_kv_cache` follow the reference's tuple convention `(kv, tokens_seen)` (T.py:2613, 2636); `kv` is a `TextKVCache`
         handle onto in-place cache slabs instead of a `(layers, 2, b, h, n, d)` tensor that is concatenated per call (T.py:969-977)."""
         raw_cache, tokens_seen = default(cache, (None, 0))
         if return_loss:
             assert not exists(raw_cache) and not return_kv_cache, 'the kv cache is a decode-time structure'
             rb = pack_text_only(text, return_loss = True)
-            res = self._run(rb, None, None, train = True, vlimit = self.num_text_tokens)
+            res = self._run(rb, None, None, train = True, vlimit = self.num_text_tokens, dropout_key = dropout_key)
             if return_hiddens:
                 return res['total'], self._hiddens_padded(rb)
             return res['total']
@@ -670,11 +685,12 @@ class Transfusion(SamplingMixin, Module):
         prob_uncond = None,
         noise = None,            # extension: list (per type) of [S_t, dim_latent] noise for deterministic parity runs
         velocity_consistency_noise = None,      # extension: same, for the EMA teacher's own draw (T.py:3388-3392 draws it with randn_like)
+        dropout_key = None,      # extension: (k0, k1) u32 key of the dropout masks (csrc/dropout.cuh) for deterministic runs; None draws one per forward
     ):
         is_decoding = exists(decoding_text_or_modality)
         if is_int_tensor(modalities):
             return self.forward_text(modalities, return_loss = return_loss and not return_embed, return_embed = return_embed, cache = cache,
-                                     return_kv_cache = return_kv_cache, return_hiddens = return_hiddens)
+                                     return_kv_cache = return_kv_cache, return_hiddens = return_hiddens, dropout_key = dropout_key)
         if is_tensor(modalities) and modalities.is_floating_point():
             assert return_loss
             return self.forward_modality(modalities, modality_type = modality_type)
@@ -724,7 +740,7 @@ class Transfusion(SamplingMixin, Module):
                     out[t].append(compact[t][inst.row0: inst.row0 + inst.length])
                 return out
             kw = dict(vel_targets = vel_targets, vel_weight = self.velocity_consistency_loss_weight) if need_velocity else {}
-            res = self._run(rb, lat, eps, train = True, text_loss_weight = self.text_loss_weight, flow_loss_weight = self.flow_loss_weight, **kw)
+            res = self._run(rb, lat, eps, train = True, text_loss_weight = self.text_loss_weight, flow_loss_weight = self.flow_loss_weight, dropout_key = dropout_key, **kw)
             total = res['total']
             self._last_batch = rb
             if not return_breakdown and not return_hiddens and not return_times:
