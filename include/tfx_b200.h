@@ -187,6 +187,14 @@ int tfx_ce_fwd_bwd(const float* logits, long long ld_logits, const int* labels, 
                    double* loss_sum, int* n_valid, int M, void* stream);
 /* flow MSE fwd+bwd (T.py:3354-3362) */
 int tfx_mse_fwd_bwd(const float* pred, long long ld_pred, const float* flow, void* dpred_bf16, long long ld_dpred, float gscale, double* sumsq, long long S, int dl, void* stream);
+/* the same with the per-instance reconstruction loss folded into dpred (replaces the recon closures of MP.py:177-194 evaluated per instance at
+   T.py:3299-3308 and averaged per type at T.py:3420-3431; forward_modality: T.py:2836-2856).  Per row: d = pred - target, r = a pred - b g with
+   a = 1 - t_row, b = t_row (b_is_t) or 1; dpred = gscale d + rscale inst_w[i] a r (bf16), sumsq += d^2, inst_sumsq[i] += r^2,
+   type_sum += inst_w[i] r^2, i = row_inst[row].  All per-instance data is on the device (CUDA-graph replay across instance splits).
+   rscale = 0 writes exactly the dpred of tfx_mse_fwd_bwd. */
+int tfx_mse_recon_fwd_bwd(const float* pred, long long ld_pred, const float* target, const float* g, const float* t_row, int b_is_t, const int* row_inst,
+                          const float* inst_w, void* dpred_bf16, long long ld_dpred, float gscale, float rscale, double* sumsq, double* inst_sumsq, double* type_sum,
+                          long long S, int dl, void* stream);
 int tfx_colsum_bf16(const void* in_bf16, long long ld, long long M, int N, const int* col_map, float* out, void* stream);
 int tfx_colsum_f32(const float* in, long long ld, long long M, int N, const int* col_map /* optional */, float* out, void* stream);
 /* all per-optimizer-step weight repacks in one launch; jobs / block tables live in device memory (built once by the host) */

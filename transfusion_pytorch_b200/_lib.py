@@ -52,6 +52,7 @@ SIGNATURES = {
     'tfx_geglu_bwd_drop': [VP, VP, VP, LL, I, VP, VP, VP, VP, F, I, VP],
     'tfx_ce_fwd_bwd': [VP, LL, VP, I, I, F, VP, LL, VP, VP, I, VP],
     'tfx_mse_fwd_bwd': [VP, LL, VP, VP, LL, F, VP, LL, I, VP],
+    'tfx_mse_recon_fwd_bwd': [VP, LL, VP, VP, VP, I, VP, VP, VP, LL, F, F, VP, VP, VP, LL, I, VP],
     'tfx_colsum_bf16': [VP, LL, LL, I, VP, VP, VP],
     'tfx_colsum_f32': [VP, LL, LL, I, VP, VP, VP],
     'tfx_cast_pack_multi': [VP, VP, VP, I, VP],

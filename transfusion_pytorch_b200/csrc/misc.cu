@@ -221,6 +221,67 @@ __global__ void mse_fwd_bwd_k(const float* __restrict__ pred, long long ld_p, co
   }
 }
 
+// flow MSE with the per-instance reconstruction loss (MP.py:177-194, T.py:3299-3308, 3420-3431; forward_modality T.py:2836-2856), forward +
+// backward in one pass over a modality type's compact rows, one warp per row:
+//   d = p - target                      (target: the flow, or the velocity blend)
+//   r = a p - b g,  a = 1 - t,  b = t (interleaved: g = flow, since noised - noise = t flow) or 1 (forward_modality: g = orig - noise)
+//   dpred = gscale d + rscale w_i a r   (bf16, written once) ;  sumsq += d^2 ;  inst_sumsq[i] += r^2 ;  type_sum += w_i r^2
+// with i = row_inst[row] and w_i = inst_w[i] = 1 / (instances of the type x rows of instance i): type_sum / dl is the type's mean of the
+// per-instance MSEs.  Instance index and weight are device data, so a captured graph replays batches with another instance split.
+// A warp walks a contiguous run of rows and flushes its partial of the current instance with one atomic whenever the instance changes.
+// SAME_G: g is the target (interleaved path without velocity): read once.
+template <bool SAME_G>
+__global__ void __launch_bounds__(256) mse_recon_fwd_bwd_k(const float* __restrict__ pred, long long ld_p, const float* __restrict__ target, const float* __restrict__ g,
+                                                          const float* __restrict__ t_row, int b_is_t, const int* __restrict__ row_inst, const float* __restrict__ inst_w,
+                                                          __nv_bfloat16* __restrict__ dpred, long long ld_d, float gscale, float rscale, double* __restrict__ sumsq,
+                                                          double* __restrict__ inst_sumsq, double* __restrict__ type_sum, long long S, int dl, long long rows_per_warp) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const long long warp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+  const long long r0 = warp * rows_per_warp, r1 = min(S, r0 + rows_per_warp);
+  float fl = 0.f, seg = 0.f, tsum = 0.f;           // flow sum of squares, recon sum of the current segment (lane partials); sum of w_i x segment (lane 0)
+  int cur = -1;
+  float cur_w = 0.f;
+  for (long long r = r0; r < r1; ++r) {
+    const int i = row_inst[r];
+    if (i != cur) {
+      if (cur >= 0) {
+        const float s = warp_sum(seg);
+        if (lane == 0) { atomicAdd(inst_sumsq + cur, (double)s); tsum += cur_w * s; }
+        seg = 0.f;
+      }
+      cur = i; cur_w = inst_w[i];
+    }
+    const float t = t_row[r], a = 1.f - t, b = b_is_t ? t : 1.f;
+    const float c = rscale * cur_w * a;
+    const float* pr = pred + r * ld_p;
+    const float* tr = target + r * dl;
+    const float* gr = g + r * dl;
+    __nv_bfloat16* dr = dpred + r * ld_d;
+    for (int col = lane; col < dl; col += 32) {
+      const float p = pr[col], f = tr[col];
+      const float gv = SAME_G ? f : gr[col];
+      const float d = p - f, rr = a * p - b * gv;
+      fl += d * d; seg += rr * rr;
+      float v = d * gscale;
+      if (c != 0.f) v = fmaf(c, rr, v);              // c = 0 (w_r = 0): exactly the dpred of mse_fwd_bwd
+      dr[col] = __float2bfloat16(v);
+    }
+  }
+  if (cur >= 0) {
+    const float s = warp_sum(seg);
+    if (lane == 0) { atomicAdd(inst_sumsq + cur, (double)s); tsum += cur_w * s; }
+  }
+  fl = warp_sum(fl);
+  __shared__ float red[2][8];
+  if (lane == 0) { red[0][w] = fl; red[1][w] = tsum; }
+  __syncthreads();
+  if (w == 0) {
+    float a = lane < (blockDim.x >> 5) ? red[0][lane] : 0.f, b = lane < (blockDim.x >> 5) ? red[1][lane] : 0.f;
+    a = warp_sum(a); b = warp_sum(b);
+    if (lane == 0) { atomicAdd(sumsq, (double)a); atomicAdd(type_sum, (double)b); }
+  }
+}
+
 // out[col_map ? col_map[c] : c] += sum_r in[r][c]    (bias gradients)
 __global__ void colsum_bf16_k(const __nv_bfloat16* __restrict__ in, long long ld, long long M, int N, const int* __restrict__ col_map, float* __restrict__ out, int rows_per_block) {
   const int cp = threadIdx.x & 31, rl = threadIdx.x >> 5;           // 32 column pairs x 8 row lanes
@@ -445,6 +506,26 @@ int tfx_mse_fwd_bwd(const float* pred, long long ld_pred, const float* flow, voi
   if (S <= 0) return 0;
   mse_fwd_bwd_k<<<ew_grid(S * dl, 256), 256, 0, ST(stream)>>>(pred, ld_pred, flow, (__nv_bfloat16*)dpred_bf16, ld_dpred, gscale, sumsq, S, dl);
   return check_launch("mse_fwd_bwd");
+}
+
+int tfx_mse_recon_fwd_bwd(const float* pred, long long ld_pred, const float* target, const float* g, const float* t_row, int b_is_t, const int* row_inst,
+                          const float* inst_w, void* dpred_bf16, long long ld_dpred, float gscale, float rscale, double* sumsq, double* inst_sumsq, double* type_sum,
+                          long long S, int dl, void* stream) {
+  if (S <= 0) return 0;
+  TFX_REQUIRE(pred && target && g && t_row && row_inst && inst_w && dpred_bf16 && sumsq && inst_sumsq && type_sum && dl > 0,
+              "mse_recon_fwd_bwd: every pointer is required and dl (%d) must be > 0", dl);
+  const int threads = 256, wpb = threads / 32;
+  long long blocks = (S + wpb - 1) / wpb;
+  const long long cap = (long long)num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  const long long warps = blocks * wpb, rpw = (S + warps - 1) / warps;
+  if (g == target)
+    mse_recon_fwd_bwd_k<true><<<(unsigned)blocks, threads, 0, ST(stream)>>>(pred, ld_pred, target, g, t_row, b_is_t, row_inst, inst_w, (__nv_bfloat16*)dpred_bf16, ld_dpred,
+                                                                          gscale, rscale, sumsq, inst_sumsq, type_sum, S, dl, rpw);
+  else
+    mse_recon_fwd_bwd_k<false><<<(unsigned)blocks, threads, 0, ST(stream)>>>(pred, ld_pred, target, g, t_row, b_is_t, row_inst, inst_w, (__nv_bfloat16*)dpred_bf16, ld_dpred,
+                                                                           gscale, rscale, sumsq, inst_sumsq, type_sum, S, dl, rpw);
+  return check_launch("mse_recon_fwd_bwd");
 }
 
 int tfx_colsum_bf16(const void* in_bf16, long long ld, long long M, int N, const int* col_map, float* out, void* stream) {

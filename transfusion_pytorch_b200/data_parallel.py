@@ -95,7 +95,8 @@ class DataParallelTrainer:
         device_lat: per-type latent matrices already on the device (then rb must be uploaded too: a device-resident batch)."""
         model, eng = self.model, self.model.engine
         drop = model.transformer.ff_dropout_p(True, model.training) > 0.
-        sig = self._signature(rb, eng) + (drop,)          # a step with dropout launches other kernels than one without
+        recon = bool(model.has_recon_loss)
+        sig = self._signature(rb, eng) + (drop, recon)     # a step with dropout / the reconstruction loss launches other kernels than one without
         g = self._graphs.get(sig)
         if g is None:
             if len(self._graphs) >= 8:
@@ -172,7 +173,7 @@ class DataParallelTrainer:
             l0 = eng.ops.launches
             with torch.cuda.graph(graph):
                 res = eng.forward(rb, g.lat, g.eps, train = True, text_loss_weight = model.text_loss_weight, flow_loss_weight = model.flow_loss_weight,
-                                  dropout = model.training, dropout_key = g.drop_key)
+                                  dropout = model.training, dropout_key = g.drop_key, recon_weight = model.reconstruction_loss_weight if recon else 0.)
                 # NCCL all-reduce of the flat gradient buffer captured INSIDE the step graph: per-layer buckets on the communication stream, forked
                 # from / joined to the capture stream, so the collective of layers >= i overlaps the backward kernels of layers < i on every replay
                 self._backward_allreduce(eng, lambda cb: eng.backward(bucket_cb = cb))

@@ -338,14 +338,15 @@ class Engine:
 
     # ------------------------------------------------------------------ descriptor upload
     META_NAMES = ['text_id', 'label', 'kv_limit', 'rope_pos', 'cond_row', 'slot', 'tile_q0', 'tile_qend', 'tile_kv0', 'tile_kvend',
-                  'kt_kv0', 'kt_kvend', 'kt_q0', 'kt_qend', 'row_token', 't2_q0', 't2_qend', 't2_kv0', 't2_kvend', 'k2_kv0', 'k2_kvend', 'k2_q0', 'k2_qend', 'k2_order', 'kv_row', 'pos_c0', 'pos_c1', 'pos_c2']
+                  'kt_kv0', 'kt_kvend', 'kt_q0', 'kt_qend', 'row_token', 't2_q0', 't2_qend', 't2_kv0', 't2_kvend', 'k2_kv0', 'k2_kvend', 'k2_q0', 'k2_qend', 'k2_order', 'kv_row', 'pos_c0', 'pos_c1', 'pos_c2',
+                  'row_inst']
 
     def stage_meta(self, rb: RaggedBatch):
         """All per-token / per-tile int32 metadata and the float metadata of a batch in ONE pooled pinned buffer.
         Returns (raw pinned buffer, int32 view, layout) - layout = (sizes per array, n_int, n_float)."""
         ints = [getattr(rb, n) if getattr(rb, n) is not None else _EMPTY_I32 for n in self.META_NAMES]
         sizes = [_round_up(a.shape[0], 4) for a in ints]
-        fl = np.concatenate([rb.cond_times, rb.row_time]).astype(np.float32)
+        fl = np.concatenate([rb.cond_times, rb.row_time] + ([rb.inst_w] if rb.inst_w is not None else [])).astype(np.float32)
         n_int, n_fl = sum(sizes), _round_up(fl.shape[0], 4)
         raw = POOL.take((n_int + n_fl) * 4)                       # pooled pinned staging: no per-step cudaHostAlloc
         host = raw[:(n_int + n_fl) * 4].view(I32)
@@ -362,7 +363,9 @@ class Engine:
         for n, ln, s in zip(self.META_NAMES, lens, sizes):
             d[n] = devbuf[off:off + ln]; off += s
         fdev = devbuf[n_int:n_int + n_fl].view(F32)
-        d['cond_times'], d['row_time'] = fdev[:rb.n_cond], fdev[rb.n_cond:]
+        d['cond_times'], d['row_time'] = fdev[:rb.n_cond], fdev[rb.n_cond:rb.n_cond + rb.S]
+        if rb.inst_w is not None:                                  # reconstruction loss: per-instance weights behind the row times
+            d['inst_w'] = fdev[rb.n_cond + rb.S:]
         d['h2d_bytes'] = devbuf.numel() * 4
         d['_keep'] = devbuf
         d['_layout'] = layout
@@ -401,12 +404,16 @@ class Engine:
     # ------------------------------------------------------------------ forward
     def forward(self, rb: RaggedBatch, latents: list | None, eps: list | None, *, train: bool, want_logits = False, vlimit = 0,
                 text_loss_weight = 1., flow_loss_weight = 1., modality_only = False, cache: KVCache | None = None, want_preds = None,
-                vel_targets = None, vel_weight = 0., dropout = False, dropout_key = None):
+                vel_targets = None, vel_weight = 0., dropout = False, dropout_key = None, vel_grad = True, recon_weight = 0., recon_g = None):
         """Runs the block stack over a ragged batch.  `latents[t]`: fp32 [S_t, dl_t] device tensors (clean latents when
         `eps` is given, already-noised / decode-time latents otherwise).  With train=True activations are kept for
         `backward()` and the fused loss heads produce the loss scalars and the head gradients in the same pass.
         `dropout`: the owning module is in training mode; FFN dropout then applies to a train forward (`Transformer.ff_dropout_p`), with the
-        masks of `dropout_key` (see `dropout_key()`)."""
+        masks of `dropout_key` (see `dropout_key()`).
+        `vel_grad = False`: the velocity term only adds its value, mse(flow, vel_target) (forward_modality, T.py:2823-2834).
+        `recon_weight > 0` (train forwards): the reconstruction loss (MP.py:177-194, T.py:3420-3431) is folded into the flow head's gradient
+        pass (tfx_mse_recon_fwd_bwd); its residual per row is (1 - t) pred - t flow, or with `recon_g` (per type, forward_modality T.py:2840-2856)
+        (1 - t) pred - g.  Needs the batch's reconstruction metadata (`modality_processing.build_recon_meta`)."""
         self.ensure_attached()
         self.pack_weights(force = train)
         o, D, HI, H, Ip, M = self.ops, self.D, self.HI, self.H, self.Ip, rb.M
@@ -613,6 +620,22 @@ class Engine:
             st['dpred'] = []
             flow_terms = []
             vel_terms = {}
+            recon_on = recon_weight > 0.
+            recon_terms = {}
+            if recon_on:
+                assert 'inst_w' in dv, 'the reconstruction loss needs the batch packed for a model with reconstruction_loss_weight > 0'
+                rsum = self.buf('reconacc', (len(self.dls),), torch.float64); rsum.zero_()
+                rinst = self.buf('reconinst', (S,), torch.float64); rinst.zero_()       # per-instance sums of squares, sized by S (graph signature)
+            def flow_grad(t, target, G, sumsq, dpred, n, dl, dlp):
+                s0 = rb.type_rows[t][0]
+                if not recon_on:
+                    o.mse_fwd_bwd(preds[t], dl, target, dpred, dlp, G, sumsq, n, dl)
+                    return
+                g = recon_g[t] if recon_g is not None and recon_g[t] is not None else st['flow'][t]
+                rs = 2.0 * recon_weight * wt / dl
+                o.mse_recon_fwd_bwd(preds[t], dl, target, g, dv['row_time'][s0:s0 + n], 0 if modality_only else 1, dv['row_inst'][s0:s0 + n], dv['inst_w'],
+                                    dpred, dlp, G, rs, sumsq, rinst, rsum[t:t + 1], n, dl)
+                recon_terms[t] = (rsum[t] / dl).float()
             for t, (s0, s1) in enumerate(rb.type_rows):
                 n = s1 - s0
                 if n == 0 or st['flow'][t] is None:
@@ -623,7 +646,15 @@ class Engine:
                 if dlp != dl:
                     dpred[:, dl:].zero_()
                 ga = 2.0 * flow_loss_weight * wt / (n * dl)
-                if vel_targets is not None and vel_targets[t] is not None and vel_weight != 0.:
+                if vel_targets is not None and vel_targets[t] is not None and not vel_grad:
+                    # value only: mse(flow, target) (forward_modality's velocity term carries no gradient, T.py:2834)
+                    vacc = self.buf('velacc', (len(self.dls),), torch.float64)
+                    if not vel_terms:
+                        vacc.zero_()
+                    o.mse_fwd_bwd(vel_targets[t], dl, st['flow'][t], None, dlp, 0., vacc[t: t + 1], n, dl)
+                    vel_terms[t] = (vacc[t] / (n * dl)).float()
+                    flow_grad(t, st['flow'][t], ga, acc[1 + t: 2 + t], dpred, n, dl, dlp)
+                elif vel_targets is not None and vel_targets[t] is not None and vel_weight != 0.:
                     # velocity consistency (T.py:3383-3418): + w_v * wt * mse(pred, ema_pred).  d/dpred of a |p - f|^2 + b |p - e|^2 is
                     # (a + b) (p - (a f + b e) / (a + b)): ONE gradient pass against the blended target; the two loss values come from two
                     # loss-only passes (their dpred output is overwritten by the blended pass)
@@ -640,10 +671,10 @@ class Engine:
                     o.axpy_f32(blend, st['flow'][t], ga / (ga + gb), n * dl)
                     o.axpy_f32(blend, e, gb / (ga + gb), n * dl)
                     scratch = self.buf('velscratch', (1,), torch.float64)
-                    o.mse_fwd_bwd(preds[t], dl, blend, dpred, dlp, ga + gb, scratch, n, dl)
+                    flow_grad(t, blend, ga + gb, scratch, dpred, n, dl, dlp)
                     vel_terms[t] = (vacc[t] / (n * dl)).float()
                 else:
-                    o.mse_fwd_bwd(preds[t], dl, st['flow'][t], dpred, dlp, ga, acc[1 + t: 2 + t], n, dl)
+                    flow_grad(t, st['flow'][t], ga, acc[1 + t: 2 + t], dpred, n, dl, dlp)
                 st['dpred'].append(dpred)
                 flow_terms.append((acc[1 + t] / (n * dl)).float() )
             # loss assembly on a handful of device scalars (no host sync): transfusion.py:3331-3376
@@ -655,6 +686,10 @@ class Engine:
                 total = text.clone()         # distinct tensor: autograd.Function outputs must not alias each other
             elif modality_only:
                 total = flows.sum()
+                for t, f in vel_terms.items():
+                    total = total + f * vel_weight
+                for t, r in recon_terms.items():
+                    total = total + r * recon_weight
             else:
                 total = (acc[0] / T).float() * text_loss_weight          # = text * (n_valid / T) * w  (T.py:3331, 3371)
                 for t, f in enumerate(flow_terms):
@@ -662,8 +697,12 @@ class Engine:
                         total = total + f * (rb.n_type_tokens[t] / T) * flow_loss_weight
                 for t, f in vel_terms.items():
                     total = total + f * (rb.n_type_tokens[t] / T) * vel_weight
+                for t, r in recon_terms.items():
+                    total = total + r * (rb.n_type_tokens[t] / T) * recon_weight
             vel = [vel_terms.get(t, torch.zeros((), device = self.device)) for t in range(len(self.dls))] if vel_terms else None
             res.update(loss_acc = acc, n_valid = nvalid, total = total, text = text, flows = flows, vel = vel)
+            if recon_on:
+                res.update(recon = [recon_terms.get(t, torch.zeros((), device = self.device)) for t in range(len(self.dls))], recon_inst = rinst)
         return res
 
     def dropout_key(self, src = None, out: Tensor | None = None) -> Tensor:

@@ -95,6 +95,8 @@ class RaggedBatch:
     pos_c1: np.ndarray = None
     pos_c2: np.ndarray = None
     pos_max: tuple = None                   # per type: per-axis table lengths (batch maximum, rounded up to a multiple of 8) or None
+    row_inst: np.ndarray = None             # reconstruction loss only: [S] index into `instances` of every compact row
+    inst_w: np.ndarray = None               # reconstruction loss only: [S] float32, entry i = 1 / (instances of i's type x rows of i); zero past the instances
     kv_row: np.ndarray = None               # kv-cache forward only: cache row each (new) token's key / value is appended at
     single_row_tiles: bool = False          # every attention tile holds exactly one query row (text decode): use the decode kernel
     max_rope_pos: int = 0
@@ -340,8 +342,31 @@ def pack_batch(
             pmax[t] = ax if pmax[t] is None else tuple(max(x, y) for x, y in zip(pmax[t], ax))
         rb.pos_c0, rb.pos_c1, rb.pos_c2 = coords
         rb.pos_max = tuple(None if m is None else tuple((x + 7) // 8 * 8 for x in m) for m in pmax)
+    if getattr(model, 'has_recon_loss', False):
+        build_recon_meta(rb)
     build_tiles(rb, qfirst)
     return rb
+
+
+def build_recon_meta(rb: RaggedBatch) -> None:
+    """Per-row instance index and per-instance weights of the reconstruction loss (T.py:3299-3308, 3420-3431): the loss of a type is the mean
+    over its instances of each instance's MSE, so instance i weighs 1 / (K_t n_i) (K_t instances of its type, n_i rows).  Both arrays are
+    sized by S, so their shapes depend only on the batch's shape signature; the values travel in the metadata upload (a replayed CUDA graph
+    reads them from the device)."""
+    S = rb.S
+    row_inst = np.zeros(S, dtype = np.int32)
+    inst_w = np.zeros(S, dtype = np.float32)
+    if rb.instances:
+        ni = len(rb.instances)
+        il = np.fromiter((i.length for i in rb.instances), dtype = np.int64, count = ni)
+        ity = np.fromiter((i.modality_type for i in rb.instances), dtype = np.int64, count = ni)
+        base = np.asarray([s0 for s0, _ in rb.type_rows], dtype = np.int64)
+        ir0 = base[ity] + np.fromiter((i.row0 for i in rb.instances), dtype = np.int64, count = ni)
+        order = np.argsort(ir0, kind = 'stable')                        # compact rows hold the instances in (type, scan) order
+        row_inst[:] = np.repeat(order, il[order])
+        k = np.bincount(ity, minlength = rb.n_types)
+        inst_w[:ni] = 1. / (k[ity] * np.maximum(il, 1))
+    rb.row_inst, rb.inst_w = row_inst, inst_w
 
 
 def pack_incremental(samples: list, times, model, *, slab: np.ndarray, base_len: np.ndarray, rope_base: np.ndarray, cap: int) -> RaggedBatch:

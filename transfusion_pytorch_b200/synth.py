@@ -130,3 +130,55 @@ def config4_batch(batch: int, seed: int = 0, **kw):
 
 def text_batch(batch: int, seq: int, vocab: int = 256, seed: int = 0) -> torch.Tensor:
     return torch.randint(0, vocab, (batch, seq), generator = _gen(31337 + seed))
+
+
+def recon_batch(dims = (32, 16), text_vocab: int = 64, seed: int = 23):
+    """Four interleaved samples with 3, 0, 1 and 2 modality instances of two types and ragged lengths (1 to 33 rows): the reconstruction-loss
+    fixtures (tests/golden/small_recon*.pt)."""
+    g = _gen(seed)
+    txt = lambda n: torch.randint(0, text_vocab, (n,), generator = g)
+    lat = lambda t, n: (t, torch.randn(n, dims[t], generator = g))
+    return [[txt(4), lat(0, 5), txt(3), lat(1, 31), txt(2), lat(0, 33), txt(5)],
+            [txt(9)],
+            [txt(6), lat(1, 1), txt(4)],
+            [lat(0, 12), txt(7), lat(1, 7), txt(3)]]
+
+
+def recon_times(seed: int = 29) -> torch.Tensor:
+    """times of `recon_batch`: one per instance slot, with one time near 0 and one near 1"""
+    t = torch.rand(4, 3, generator = _gen(seed))
+    t[0, 0], t[3, 1] = 0.02, 0.97
+    return t
+
+
+def modality_batch(batch: int = 3, length: int = 9, dim: int = 32, seed: int = 41) -> torch.Tensor:
+    """[batch, length, dim] modalities for `forward_modality` (reconstruction / velocity fixtures)"""
+    return torch.randn(batch, length, dim, generator = _gen(seed))
+
+
+class StandInEncoder(torch.nn.Module):
+    """Small deterministic modality encoder (a fixed Linear then tanh) standing in for a VAE encoder in the reconstruction-loss fixtures"""
+
+    def __init__(self, dim_in: int, dim_latent: int, seed: int = 51):
+        super().__init__()
+        self.proj = torch.nn.Linear(dim_in, dim_latent)
+        with torch.no_grad():
+            self.proj.weight.copy_(torch.randn(dim_latent, dim_in, generator = _gen(seed)) * dim_in ** -0.5)
+            self.proj.bias.copy_(torch.randn(dim_latent, generator = _gen(seed + 1)) * 0.1)
+
+    def forward(self, x):
+        return torch.tanh(self.proj(x))
+
+
+class StandInDecoder(torch.nn.Module):
+    """Decoder paired with `StandInEncoder`: a fixed Linear from the latent back to the modality's width"""
+
+    def __init__(self, dim_latent: int, dim_out: int, seed: int = 53):
+        super().__init__()
+        self.proj = torch.nn.Linear(dim_latent, dim_out)
+        with torch.no_grad():
+            self.proj.weight.copy_(torch.randn(dim_out, dim_latent, generator = _gen(seed)) * dim_latent ** -0.5)
+            self.proj.bias.copy_(torch.randn(dim_out, generator = _gen(seed + 1)) * 0.1)
+
+    def forward(self, x):
+        return self.proj(x)

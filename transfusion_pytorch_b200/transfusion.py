@@ -7,8 +7,7 @@ versa.  What differs is everything underneath: the modules below only OWN parame
 the block stack, attention, loss heads and optimizer runs in the sm_90a kernels of `libtfx_b200.so`
 driven by `engine.Engine` over the ragged descriptor of `modality_processing.pack_batch`.
 
-Out of scope here (SURVEY.md section 2 rows 16-23, raise loudly): axial positional embeddings, U-Net
-pre/post encoders, velocity-consistency / reconstruction losses, LASER attention, value residual.
+Out of scope here (raise loudly): U-Net pre/post encoders (`pre_post_transformer_enc_dec`), attention dropout, dim_head != 64.
 """
 from __future__ import annotations
 
@@ -256,6 +255,7 @@ class _TrainStep(torch.autograd.Function):
         res = engine.forward(rb, latents, eps, train = True, **kw)
         ctx.engine = engine
         engine._last_vel = res.get('vel')
+        engine._last_res = res
         return res['total'], res['text'], res['flows']
 
     @staticmethod
@@ -302,7 +302,6 @@ class Transfusion(SamplingMixin, Module):
 
         self.model_output_clean = bool(model_output_clean)
         if exists(pre_post_transformer_enc_dec): raise NotImplementedError('pre_post_transformer_enc_dec (U-Net) is outside the CUDA hot path')
-        if reconstruction_loss_weight > 0.: raise NotImplementedError('reconstruction loss is outside the CUDA hot path')
         assert ignore_index == -1, 'the fused loss kernel uses -1 as the ignore index'
 
         self.dim_latents = cast_tuple(default(dim_latent, dim))
@@ -361,7 +360,8 @@ class Transfusion(SamplingMixin, Module):
         self.ignore_index = ignore_index
         self.flow_loss_weight, self.text_loss_weight = flow_loss_weight, text_loss_weight
         self.velocity_consistency_loss_weight = velocity_consistency_loss_weight
-        self.has_recon_loss, self.reconstruction_loss_weight = False, reconstruction_loss_weight
+        # reconstruction loss (MP.py:177-194, T.py:3420-3431, 2836-2856): folded into the flow head's gradient pass (tfx_mse_recon_fwd_bwd)
+        self.has_recon_loss, self.reconstruction_loss_weight = reconstruction_loss_weight > 0., reconstruction_loss_weight
         self.model_output_clean, self.eps = model_output_clean, eps
         self.odeint_kwargs = dict(odeint_kwargs)
         assert self.odeint_kwargs.get('method', 'midpoint') == 'midpoint', 'only the fixed-grid midpoint solver is implemented'
@@ -482,11 +482,28 @@ class Transfusion(SamplingMixin, Module):
         eng = self.engine
         if self.transformer.ff_dropout_p(train, self.training) > 0.:
             kw.update(dropout = True, dropout_key = dropout_key)
+        if train and self.has_recon_loss and rb.inst_w is not None:
+            kw.setdefault('recon_weight', self.reconstruction_loss_weight)
         if train and torch.is_grad_enabled():
             anchor = self.text_embed.weight
             total, text, flows = _TrainStep.apply(eng, rb, latents, eps, kw, anchor)
-            return dict(total = total, text = text, flows = flows, vel = eng._last_vel)
+            last = eng._last_res
+            return dict(total = total, text = text, flows = flows, vel = eng._last_vel, recon = last.get('recon'), recon_inst = last.get('recon_inst'), preds = last.get('preds'))
         return eng.forward(rb, latents, eps, train = train, **kw)
+
+    def _recon_breakdown(self, rb, res):
+        """`LossBreakdown.recon` (T.py:3288-3311, 3441): per modality type (all of them, absent ones included) the list of per-instance reconstruction
+        MSEs in scan order; device scalars, no host synchronisation"""
+        out = [[] for _ in range(self.num_modalities)]
+        inst = res.get('recon_inst')
+        if inst is None or not rb.instances:
+            return out
+        ni = len(rb.instances)
+        denom = np.fromiter((i.length * self.dim_latents[i.modality_type] for i in rb.instances), dtype = np.float64, count = ni)
+        vals = (inst[:ni] / torch.from_numpy(denom).to(inst.device, non_blocking = True)).float()
+        for k, i in enumerate(rb.instances):
+            out[i.modality_type].append(vals[k])
+        return out
 
     def forward_packed(self, rb: RaggedBatch, latents: list, noise: list | None = None, return_breakdown = False, dropout_key = None):
         """Training step from an already packed (and possibly already uploaded) ragged batch: the part of `forward`
@@ -495,7 +512,8 @@ class Transfusion(SamplingMixin, Module):
         res = self._run(rb, latents, eps, train = True, text_loss_weight = self.text_loss_weight, flow_loss_weight = self.flow_loss_weight, dropout_key = dropout_key)
         self._last_batch = rb
         if return_breakdown:
-            return res['total'], LossBreakdown(res['total'], res['text'], list(res['flows']), None, None)
+            recon = self._recon_breakdown(rb, res) if self.has_recon_loss else None
+            return res['total'], LossBreakdown(res['total'], res['text'], list(res['flows']), None, recon)
         return res['total']
 
     # ------------------------------------------------------------------ text only (transfusion.py:2585-2707)
@@ -583,11 +601,15 @@ class Transfusion(SamplingMixin, Module):
     # ------------------------------------------------------------------ modality only (transfusion.py:2709-2866)
     def forward_modality(self, modalities: Tensor, times = None, modality_type = None, encode_modality = True, velocity_consistency_ema_model = None,
                          velocity_consistency_delta_time = 1e-5, return_loss = True, return_loss_breakdown = False, noise = None):
-        assert not exists(velocity_consistency_ema_model), 'velocity consistency is outside the CUDA hot path'
+        """T.py:2709-2866.  Training returns flow + w_v velocity + w_r recon, and with `return_loss_breakdown` (flow, velocity, recon).
+        Velocity consistency: the student runs at t (1 - delta), the EMA model predicts at t + delta on the clean encoded tokens, and the term
+        mse(flow, ema prediction) adds its value only.  Reconstruction: noise + pred (1 - t) against the input before the encoder; through a
+        `modality_decoder` (user module, run under no_grad) it adds its value only, otherwise it is fused into the flow head's gradient pass."""
         if self.num_modalities > 1:
             assert exists(modality_type), '`modality_type` must be explicitly passed in on forward when training on greater than 1 modality'
         mt = default(modality_type, 0)
-        enc = self.modality_encoder[mt]
+        enc, dec = self.modality_encoder[mt], self.modality_decoder[mt]
+        orig = modalities
         x = modalities
         if encode_modality and exists(enc):
             with torch.no_grad():
@@ -595,6 +617,20 @@ class Transfusion(SamplingMixin, Module):
         B = x.shape[0]
         if times is None:
             times = torch.rand((B,))
+        ema = velocity_consistency_ema_model if return_loss else None
+        vel_target = None
+        if exists(ema):
+            if hasattr(ema, 'ema_model'):
+                assert isinstance(ema.ema_model, Transfusion)
+                if hasattr(ema, '_engines'):
+                    ema._engines()
+                ema = ema.ema_model
+            orig_times = times.clone()
+            times = times * (1. - velocity_consistency_delta_time)        # T.py:2753-2755
+            with torch.no_grad():
+                ema.eval()
+                vel_target = ema.forward_modality(x, modality_type = mt, times = orig_times + velocity_consistency_delta_time, encode_modality = False, return_loss = False)
+            vel_target = self._modality_rows(vel_target, mt)
         samples = [[(mt, x[b])] for b in range(B)]
         rb = pack_batch(samples, times.reshape(B, 1), self, return_loss = False, return_embed = True)
         rb.kv_limit[:] = np.repeat(rb.cu[1:] - 1, rb.seq_lens).astype(np.int32)      # no mask at all (transfusion.py:2800-2804)
@@ -606,20 +642,53 @@ class Transfusion(SamplingMixin, Module):
             eps = [None] * self.num_modalities
             eps[mt] = noise.reshape(-1, self.dim_latents[mt]).float().to(self.device) if exists(noise) else torch.randn_like(lat[mt])
             rb.has_labels = True
-            res = self._run(rb, lat, eps, train = True, modality_only = True, flow_loss_weight = 1.)
+            kw = {}
+            if exists(vel_target):
+                kw.update(vel_targets = [vel_target if t == mt else None for t in range(self.num_modalities)], vel_weight = self.velocity_consistency_loss_weight, vel_grad = False)
+            fused_recon = self.has_recon_loss and not exists(dec)
+            if self.has_recon_loss:
+                assert encode_modality, 'the reconstruction loss compares with the modality before the encoder (T.py:2841)'
+                if fused_recon and exists(enc):      # residual (1 - t) pred - (orig - noise)
+                    o = self._modality_rows(orig.to(self.device), mt)
+                    if o.shape != eps[mt].shape:
+                        raise ValueError(f'reconstruction loss without a decoder: the modality before the encoder {tuple(orig.shape)} must have the shape of the encoded one {tuple(x.shape)}')
+                    g = [None] * self.num_modalities
+                    g[mt] = o - eps[mt]
+                    kw['recon_g'] = g
+                kw['recon_weight'] = self.reconstruction_loss_weight if fused_recon else 0.
+            res = self._run(rb, lat, eps, train = True, modality_only = True, flow_loss_weight = 1., **kw)
             flow_loss = res['flows'][mt]
             total = res['total']
+            velocity_loss = res['vel'][mt] if exists(vel_target) else self.zero
+            recon_loss = res['recon'][mt] if fused_recon else self.zero
+            if self.has_recon_loss and exists(dec):
+                # decoder(noise + pred (1 - t)) under no_grad (T.py:2843-2848): adds to the value, carries no gradient
+                with torch.no_grad():
+                    s0, s1 = rb.type_rows[mt]
+                    tr = rb.dev['row_time'][s0:s1, None] if rb.dev else torch.as_tensor(rb.row_time[s0:s1])[:, None]
+                    rec = eps[mt] + res['preds'][mt] * (1. - tr)
+                    dec.eval()
+                    out = dec(self._rows_to_modality(rec, x, mt))
+                    recon_loss = torch.nn.functional.mse_loss(out.float(), orig.to(out.device).float())
+                total = total + recon_loss * self.reconstruction_loss_weight
             if return_loss_breakdown:
-                return total, (flow_loss, self.zero, self.zero)
+                return total, (flow_loss, velocity_loss, recon_loss)
             return total
         res = self.engine.forward(rb, lat, None, train = False, want_logits = True)
-        pred = res['preds'][mt]
-        cf = self.channel_first_latent[mt]
-        inst_shape = x.shape[2:] if cf else x.shape[1:-1]
-        pred = pred.reshape(B, *inst_shape, self.dim_latents[mt])
-        if cf:
-            pred = pred.movedim(-1, 1)
-        return pred
+        return self._rows_to_modality(res['preds'][mt], x, mt)
+
+    def _rows_to_modality(self, rows, like, mt):
+        """[B * n, dim_latent] compact rows -> the layout of `like` ([B, *axial, d] or channel first [B, d, *axial])"""
+        B, cf = like.shape[0], self.channel_first_latent[mt]
+        inst_shape = like.shape[2:] if cf else like.shape[1:-1]
+        out = rows.reshape(B, *inst_shape, self.dim_latents[mt])
+        return out.movedim(-1, 1) if cf else out
+
+    def _modality_rows(self, t, mt):
+        """inverse of `_rows_to_modality`: a fresh fp32 [B * n, dim_latent] matrix on the model's device"""
+        if self.channel_first_latent[mt]:
+            t = t.movedim(1, -1)
+        return t.reshape(-1, self.dim_latents[mt]).float().to(self.device).clone()
 
     # ------------------------------------------------------------------ host side of forward(): CFG dropout, encoders, times, pack / route
     def pack(self, modalities, times = None, num_modalities_to_times_fn = None, prob_uncond = None, return_loss = True, return_embed = False, is_decoding = False):
@@ -749,7 +818,7 @@ class Transfusion(SamplingMixin, Module):
             if return_breakdown:
                 flows = [res['flows'][t] for t in range(self.num_modalities) if rb.type_rows[t][1] > rb.type_rows[t][0]]
                 vel = [res['vel'][t] for t in range(self.num_modalities) if rb.type_rows[t][1] > rb.type_rows[t][0]] if need_velocity else None
-                ret = (*ret, LossBreakdown(total, res['text'], flows, vel, [[] for _ in range(self.num_modalities)]))
+                ret = (*ret, LossBreakdown(total, res['text'], flows, vel, self._recon_breakdown(rb, res)))
             if return_hiddens:
                 ret = (*ret, self._hiddens_padded(rb))
             if return_times:
