@@ -156,6 +156,13 @@ int tfx_attn_residual_bwd_h16(const void* const* hiddens_bf16, float* const* dhi
 /* final RMSNorm (T.py:1250, 785-786) (+ compaction of modality rows for the flow head) */
 int tfx_rmsnorm_fwd(const float* x, const float* gamma, float* out_f32, void* out_bf16, const int* slot, void* out_mod_bf16, int M, int D, void* stream);
 int tfx_rmsnorm_bwd(const float* dout, const float* x, const float* gamma, float* dx, float* dgamma, int M, int D, void* stream);
+/* Self-Flow representation loss (T.py:3458-3460): loss = 1 - mean over the M rows of cosine_similarity(a_r, b_r), norms clamped to 1e-8 each
+ * (torch.nn.functional.cosine_similarity), written to `loss` (float, device); in the same pass da = d(g * loss)/da in bf16, g a device scalar,
+ * the mean taken over n_mean rows.  a fp32 [M][D]; b [M][D], bf16 if b_bf16 else fp32.  partials: tfx_rep_cos_blocks(M) doubles; ticket: one
+ * zero-initialised u32 the kernel leaves at zero.  The sum is deterministic for a given M and GPU. */
+int tfx_rep_cos_blocks(int M);
+int tfx_rep_cos_fwd_bwd(const float* a, const void* b, int b_bf16, const float* g, int n_mean, void* da_bf16, double* partials, unsigned int* ticket, float* loss,
+                        int M, int D, void* stream);
 /* token assemble: where(is_modality, modality_token, text_embed[id]) (T.py:3173-3184) and its backward */
 int tfx_embed_assemble(const int* text_id, const float* emb, const float* modtok, const int* slot, float* x0, void* x0_bf16, int M, int D, void* stream);
 int tfx_embed_bwd(const float* dx0, const int* text_id, const int* slot, float* demb, void* dmodtok_bf16, int M, int D, void* stream);

@@ -42,6 +42,7 @@ SIGNATURES = {
     'tfx_attn_residual_bwd_h16': [VP, VP, I, VP, VP, VP, VP, VP, VP, VP, VP, I, I, I, VP],
     'tfx_rmsnorm_fwd': [VP, VP, VP, VP, VP, VP, I, I, VP],
     'tfx_rmsnorm_bwd': [VP, VP, VP, VP, VP, I, I, VP],
+    'tfx_rep_cos_fwd_bwd': [VP, VP, I, VP, I, VP, VP, VP, VP, I, I, VP],
     'tfx_embed_assemble': [VP, VP, VP, VP, VP, VP, I, I, VP],
     'tfx_embed_bwd': [VP, VP, VP, VP, VP, I, I, VP],
     'tfx_scatter_add_rows': [VP, VP, VP, I, I, VP],
@@ -81,7 +82,7 @@ SIGNATURES = {
     'tfx_add_f32_into_bf16': [VP, LL, VP, LL, I, I, VP],
 }
 
-EXPORTED = ['tfx_last_error', 'tfx_version', 'tfx_geglu_bwd_rows_per_block', 'tfx_attn_residual_bwd_workspace_floats'] + list(SIGNATURES)
+EXPORTED = ['tfx_last_error', 'tfx_version', 'tfx_geglu_bwd_rows_per_block', 'tfx_attn_residual_bwd_workspace_floats', 'tfx_rep_cos_blocks'] + list(SIGNATURES)
 
 
 class TfxError(RuntimeError):
@@ -111,6 +112,8 @@ def load():
     lib.tfx_geglu_bwd_rows_per_block.argtypes = []
     lib.tfx_attn_residual_bwd_workspace_floats.restype = c_longlong
     lib.tfx_attn_residual_bwd_workspace_floats.argtypes = [c_int, c_int]
+    lib.tfx_rep_cos_blocks.restype = c_int
+    lib.tfx_rep_cos_blocks.argtypes = [c_int]
     for name, argtypes in SIGNATURES.items():
         fn = getattr(lib, name)
         fn.argtypes = argtypes

@@ -651,6 +651,56 @@ __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_bwd_k(const float* __rest
   red_row_f32<NCH>(dgamma, lane, acc);
 }
 
+// ------------------------------------------------------------------------------------ Self-Flow representation loss
+// loss = 1 - mean_r cos(a_r, b_r) (T.py:3458-3460) with the eps of torch.nn.functional.cosine_similarity: each norm is clamped to 1e-8 on its own,
+// and the clamp is a constant for the gradient.  One pass reads a and b once and writes
+//   da_r = -(g / n) (b_r / (na nb) - cos_r a_r / (na |a_r|)),   na = max(|a_r|, eps), nb = max(|b_r|, eps)   (second term 0 for a zero row),
+// g a device scalar.  The cosine sum is deterministic: per-block partials in fixed row order, summed in block order by the last block.
+template <int NCH, bool BB16>
+__global__ void __launch_bounds__(ROW_THREADS) rep_cos_fwd_bwd_k(const float* __restrict__ a, const void* __restrict__ b, const float* __restrict__ g, int n_mean,
+                                                                __nv_bfloat16* __restrict__ da, double* __restrict__ partials, unsigned int* __restrict__ ticket,
+                                                                float* __restrict__ loss, int M) {
+  constexpr int D = NCH * 128;
+  __shared__ double red[WARPS_PER_BLOCK];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+  const float gs = -__ldg(g) / (float)n_mean;
+  double local = 0.0;
+  for (int row = warp0; row < M; row += nwarps) {
+    float x[NCH * 4], y[NCH * 4];
+    load_row_f32<NCH>(a + (long long)row * D, lane, x);
+    if constexpr (BB16) load_row_bf16<NCH>(reinterpret_cast<const __nv_bfloat16*>(b) + (long long)row * D, lane, y);
+    else load_row_f32<NCH>(reinterpret_cast<const float*>(b) + (long long)row * D, lane, y);
+    float saa = 0.f, sbb = 0.f, sab = 0.f;
+#pragma unroll
+    for (int i = 0; i < NCH * 4; ++i) { saa += x[i] * x[i]; sbb += y[i] * y[i]; sab += x[i] * y[i]; }
+    const float la = sqrtf(warp_sum(saa)), lb = sqrtf(warp_sum(sbb));
+    const float na = fmaxf(la, 1e-8f), nb = fmaxf(lb, 1e-8f);
+    const float cs = warp_sum(sab) / (na * nb);
+    const float cb = gs / (na * nb), ca = la > 0.f ? -gs * cs / (na * la) : 0.f;
+#pragma unroll
+    for (int i = 0; i < NCH * 4; ++i) x[i] = cb * y[i] + ca * x[i];
+    store_row_bf16<NCH>(da + (long long)row * D, lane, x);
+    local += (double)cs;
+  }
+  if (lane == 0) red[wib] = local;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < WARPS_PER_BLOCK; ++w) s += red[w];
+    partials[blockIdx.x] = s;
+    __threadfence();
+    if (atomicAdd(ticket, 1u) == gridDim.x - 1) {
+      __threadfence();
+      double t = 0.0;
+      for (int k = 0; k < (int)gridDim.x; ++k) t += reinterpret_cast<volatile double*>(partials)[k];
+      *loss = (float)(1.0 - t / (double)n_mean);
+      *ticket = 0u;                                // ready for the next launch
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------ token assemble (+ backward)
 // x0 = isM ? modality_token[slot] : text_embed[max(id,0)]         (T.py:3173-3184)
 template <int NCH>
@@ -1005,6 +1055,18 @@ int tfx_rmsnorm_bwd(const float* dout, const float* x, const float* gamma, float
   const int tpw = 16;
   TFX_DISPATCH_NCH(D, (rmsnorm_bwd_k<NCH><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dout, x, gamma, dx, dgamma, M, tpw)));
   return check_launch("rmsnorm_bwd");
+}
+
+int tfx_rep_cos_blocks(int M) { return row_grid(M, num_sms()); }
+
+int tfx_rep_cos_fwd_bwd(const float* a, const void* b, int b_bf16, const float* g, int n_mean, void* da_bf16, double* partials, unsigned int* ticket, float* loss,
+                        int M, int D, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(n_mean > 0, "rep_cos_fwd_bwd: n_mean must be positive (got %d)", n_mean);
+  const int blocks = row_grid(M, num_sms());
+  if (b_bf16) TFX_DISPATCH_NCH(D, (rep_cos_fwd_bwd_k<NCH, true><<<blocks, ROW_THREADS, 0, ST(stream)>>>(a, b, g, n_mean, (__nv_bfloat16*)da_bf16, partials, ticket, loss, M)));
+  else TFX_DISPATCH_NCH(D, (rep_cos_fwd_bwd_k<NCH, false><<<blocks, ROW_THREADS, 0, ST(stream)>>>(a, b, g, n_mean, (__nv_bfloat16*)da_bf16, partials, ticket, loss, M)));
+  return check_launch("rep_cos_fwd_bwd");
 }
 
 int tfx_embed_assemble(const int* text_id, const float* emb, const float* modtok, const int* slot, float* x0, void* x0_bf16, int M, int D, void* stream) {

@@ -73,6 +73,52 @@ def posemb_backward(d_rows: Tensor, tables, coords, params, grads):
         gb0 += d_pre.sum(0)
 
 
+def pack_job_table(jobs, device):
+    """device job table of `tfx_cast_pack_multi` for jobs (src, ld_src, c_src, row_src, dst, r_dst, c_dst, dst_is_f32):
+    returns (table, block -> job, first block of each job, number of blocks)"""
+    # struct TfxPackJob (include/tfx_b200.h): 56 bytes
+    dt = np.dtype([('src', '<u8'), ('ld_src', '<i8'), ('row_src', '<u8'), ('dst', '<u8'), ('R_dst', '<i8'), ('C_src', '<i4'), ('C_dst', '<i4'),
+                   ('dst_f32', '<i4'), ('pad', '<i4')])
+    assert dt.itemsize == 56
+    tab = np.zeros(len(jobs), dtype = dt)
+    blk_job, blk_first = [], []
+    for j, (src, ld_src, c_src, row_src, d, r_dst, c_dst, f32) in enumerate(jobs):
+        tab[j] = (src.data_ptr(), ld_src, row_src.data_ptr() if row_src is not None else 0, d.data_ptr(), r_dst, c_src, c_dst, f32, 0)
+        nb = (r_dst * c_dst + 2047) // 2048
+        blk_first.append(len(blk_job))
+        blk_job.extend([j] * nb)
+    return (torch.from_numpy(tab.view(np.uint8).copy()).to(device), torch.tensor(blk_job, dtype = I32, device = device),
+            torch.tensor(blk_first, dtype = I32, device = device), len(blk_job))
+
+
+def w1_row_src(inner: int) -> np.ndarray:
+    """packed FeedForward W1 (GEGLU epilogue layout): tile t = [value rows 64t.. | gate rows inner+64t..]; source row of every packed row, -1 past `inner`"""
+    Ip = _round_up(inner, 64)
+    src = np.full(2 * Ip, -1, dtype = np.int64)
+    for t in range(Ip // 64):
+        for j in range(64):
+            c = 64 * t + j
+            if c < inner:
+                src[128 * t + j] = c
+                src[128 * t + 64 + j] = inner + c
+    return src
+
+
+def wgrad_splits(n_out, n_in, K, sms, ks):
+    """split-K factor of a wgrad GEMM over K tokens: tiles x splits should fill whole waves of the persistent grid (one CTA per SM); `ks` breaks
+    near-ties.  E.g. the [1408 x 512] FFN-out gradient has 22 tiles: 16 splits = 2.4 waves (80 % busy), 20 splits = 2.97 waves"""
+    tiles = ((n_out + 127) // 128) * ((n_in + 255) // 256 if (n_in % 256 == 0 or n_in >= 1024) else (n_in + 127) // 128)
+    best, best_eff = 1, 0.0
+    for s in range(1, 65):
+        if K // s < 1024 and s > 1:
+            break
+        items = tiles * s
+        eff = items / (-(-items // sms) * sms)
+        if eff > best_eff + 0.02 or (abs(eff - best_eff) <= 0.02 and s <= ks and s > best):
+            best, best_eff = s, eff
+    return best
+
+
 class KVCache:
     """Slab kv cache (decode path; reference layout `(layers, 2, batch, heads, seq, dim_head)`, T.py:976-977, 1264, 2260, re-padded and
     concatenated per step there).  Here: per layer one K (post-RoPE) and one V matrix, bf16 `[n_slabs * cap, heads * 64]`, token-major like
@@ -200,14 +246,7 @@ class Engine:
     def _build_maps(self):
         """Row maps between packed bf16 operand layouts and the state-dict parameter layouts."""
         dev, D, HI, H, inner, Ip = self.device, self.D, self.HI, self.H, self.inner, self.Ip
-        # W1 packed: tile t = [value rows 64t.. | gate rows inner+64t..]; rows past `inner` are padding
-        src = np.full(2 * Ip, -1, dtype = np.int64)
-        for t in range(Ip // 64):
-            for j in range(64):
-                c = 64 * t + j
-                if c < inner:
-                    src[128 * t + j] = c
-                    src[128 * t + 64 + j] = inner + c
+        src = w1_row_src(inner)
         self.w1_row_src = torch.from_numpy(src.astype(np.int32)).to(dev)
         self.w1_row_src64 = torch.from_numpy(src).to(dev)
         self.layer_maps = []
@@ -300,21 +339,7 @@ class Engine:
             job(self.P(f'{pre}.to_ada_ln_zero.weight'), 4 * D, 4 * D, None, wfz[w * 3 * D + 2 * D:], D, 4 * D)
             job(self.P(f'{pre}.to_film.bias'), 2 * D, 2 * D, None, bfz[w * 3 * D:], 1, 2 * D)
             job(self.P(f'{pre}.to_ada_ln_zero.bias'), D, D, None, bfz[w * 3 * D + 2 * D:], 1, D)
-        # struct TfxPackJob (include/tfx_b200.h): 56 bytes
-        dt = np.dtype([('src', '<u8'), ('ld_src', '<i8'), ('row_src', '<u8'), ('dst', '<u8'), ('R_dst', '<i8'), ('C_src', '<i4'), ('C_dst', '<i4'),
-                       ('dst_f32', '<i4'), ('pad', '<i4')])
-        assert dt.itemsize == 56
-        tab = np.zeros(len(jobs), dtype = dt)
-        blk_job, blk_first = [], []
-        for j, (src, ld_src, c_src, row_src, d, r_dst, c_dst, f32) in enumerate(jobs):
-            tab[j] = (src.data_ptr(), ld_src, row_src.data_ptr() if row_src is not None else 0, d.data_ptr(), r_dst, c_src, c_dst, f32, 0)
-            nb = (r_dst * c_dst + 2047) // 2048
-            blk_first.append(len(blk_job))
-            blk_job.extend([j] * nb)
-        self._pack_tab = torch.from_numpy(tab.view(np.uint8).copy()).to(self.device)
-        self._pack_blk_job = torch.tensor(blk_job, dtype = I32, device = self.device)
-        self._pack_blk_first = torch.tensor(blk_first, dtype = I32, device = self.device)
-        self._pack_nblocks = len(blk_job)
+        self._pack_tab, self._pack_blk_job, self._pack_blk_first, self._pack_nblocks = pack_job_table(jobs, self.device)
         self._pack_ptr = self._first_ptr
 
     def pack_weights(self, force = False):
@@ -404,7 +429,7 @@ class Engine:
     # ------------------------------------------------------------------ forward
     def forward(self, rb: RaggedBatch, latents: list | None, eps: list | None, *, train: bool, want_logits = False, vlimit = 0,
                 text_loss_weight = 1., flow_loss_weight = 1., modality_only = False, cache: KVCache | None = None, want_preds = None,
-                vel_targets = None, vel_weight = 0., dropout = False, dropout_key = None, vel_grad = True, recon_weight = 0., recon_g = None):
+                vel_targets = None, vel_weight = 0., dropout = False, dropout_key = None, vel_grad = True, recon_weight = 0., recon_g = None, rep_layer = None):
         """Runs the block stack over a ragged batch.  `latents[t]`: fp32 [S_t, dl_t] device tensors (clean latents when
         `eps` is given, already-noised / decode-time latents otherwise).  With train=True activations are kept for
         `backward()` and the fused loss heads produce the loss scalars and the head gradients in the same pass.
@@ -413,13 +438,16 @@ class Engine:
         `vel_grad = False`: the velocity term only adds its value, mse(flow, vel_target) (forward_modality, T.py:2823-2834).
         `recon_weight > 0` (train forwards): the reconstruction loss (MP.py:177-194, T.py:3420-3431) is folded into the flow head's gradient
         pass (tfx_mse_recon_fwd_bwd); its residual per row is (1 - t) pred - t flow, or with `recon_g` (per type, forward_modality T.py:2840-2856)
-        (1 - t) pred - g.  Needs the batch's reconstruction metadata (`modality_processing.build_recon_meta`)."""
+        (1 - t) pred - g.  Needs the batch's reconstruction metadata (`modality_processing.build_recon_meta`).
+        `rep_layer` (Self-Flow, `SelfMaskedRepTraining`): index into the hidden states [tokens, layer 1 .. depth, final norm]; `res['rep']` is that
+        state in packed rows.  A train forward hands it out in fp32 and `backward(g_rep = ...)` takes its gradient; an inference forward (the
+        teacher) returns the kept buffer itself and applies FFN dropout like a train forward (its module follows the wrapper's `.train()`)."""
         self.ensure_attached()
         self.pack_weights(force = train)
         o, D, HI, H, Ip, M = self.ops, self.D, self.HI, self.H, self.Ip, rb.M
         dv = self.upload(rb)
         nc, S = rb.n_cond, rb.S
-        p_ff = self.model.transformer.ff_dropout_p(train, dropout)
+        p_ff = self.model.transformer.ff_dropout_p(train or rep_layer is not None, dropout)
         st = self.state = dict(rb = rb, train = train, layers = [], p_ff = p_ff, drop_key = self.dropout_key(dropout_key) if p_ff > 0. else None)
         pk = self.packed
         rope = self.rope_table(rb.max_rope_pos)
@@ -587,6 +615,12 @@ class Engine:
             o.clean_flow_fwd(out, dv['row_token'], modtok, dv['cond_times'], dv['cond_row'], self.clean_eps, omod, S, D)
         st.update(out = out, outb = outb, omod = omod)
         res = dict(embed = out)
+        if rep_layer is not None:
+            h = (*hid, out)[rep_layer]
+            if train and h.dtype != F32:                 # the predictor head's RMSNorm reads fp32 rows
+                h = self.buf('rep_f32', (M, D), F32).copy_(h)
+            st['rep_layer'] = rep_layer
+            res['rep'] = h
 
         # ---- heads
         if want_logits or train:
@@ -735,13 +769,18 @@ class Engine:
             p.grad = gv
 
     # ------------------------------------------------------------------ backward
-    def backward(self, gscale = None, bucket_cb = None):
+    def backward(self, gscale = None, bucket_cb = None, g_rep = None):
         """Backward of the last train forward: gradients are ACCUMULATED into the flat gradient buffer
         (`param.grad` views).  All weight gradients are split-K wgmma GEMMs over the token dimension.
         `gscale`: device scalar d(loss) handed in by autograd (folded into the head gradients, no host sync).
-        `bucket_cb(layer)`: called after the kernels of a layer have been enqueued (gradient bucket ready)."""
+        `bucket_cb(layer)`: called after the kernels of a layer have been enqueued (gradient bucket ready).
+        `g_rep`: fp32 [M, D] gradient of the hidden state the forward handed out (`rep_layer`), added where that state's gradient is complete."""
         st = self.state
         assert st['train'], 'backward() needs a train forward'
+        rep_at = None
+        if g_rep is not None:
+            rep_at = st.get('rep_layer')
+            assert rep_at is not None and g_rep.dtype == F32 and g_rep.is_contiguous() and g_rep.shape == (st['rb'].M, self.D), 'g_rep: fp32 [M, D] of a rep_layer forward'
         self._prepare_grads()
         self._grads_clean = False
         self._dirty = True                      # an optimizer step (ours or torch.optim's) normally follows
@@ -759,18 +798,7 @@ class Engine:
         ks = max(1, min(64, M // 2048))           # default split-K factor of the wgrad GEMMs (K = tokens)
         sms = torch.cuda.get_device_properties(self.device).multi_processor_count
         def ksplit(n_out, n_in, K = M):
-            # split-K factor of a wgrad GEMM: tiles x splits should fill whole waves of the persistent grid (one CTA per SM);
-            # e.g. the [1408 x 512] FFN-out gradient has 22 tiles: 16 splits = 2.4 waves (80 % busy), 20 splits = 2.97 waves
-            tiles = ((n_out + 127) // 128) * ((n_in + 255) // 256 if (n_in % 256 == 0 or n_in >= 1024) else (n_in + 127) // 128)
-            best, best_eff = 1, 0.0
-            for s in range(1, 65):
-                if K // s < 1024 and s > 1:
-                    break
-                items = tiles * s
-                eff = items / (-(-items // sms) * sms)
-                if eff > best_eff + 0.02 or (abs(eff - best_eff) <= 0.02 and s <= ks and s > best):
-                    best, best_eff = s, eff
-            return best
+            return wgrad_splits(n_out, n_in, K, sms, ks)
         def wgrad(dy, ld_dy, n_out, act, ld_act, n_in, gname, K = M):
             # dW[n_out, n_in] += dy^T act : both operands MN-major over the token (K) dimension, split-K atomics
             o.gemm_store(dy, ld_dy, 1, act, ld_act, 1, n_out, n_in, K, self.G(gname), n_in, None, 0, None, None, 1.0, 1, ksplit(n_out, n_in, K))
@@ -800,6 +828,8 @@ class Engine:
                 o.clean_flow_bwd(dmod, dneg, dv['row_token'], dv['cond_times'], dv['cond_row'], self.clean_eps, S, D)
             if any_flow:
                 o.scatter_add_rows(d_out, dmod, dv['row_token'], S, D)
+        if rep_at == self.depth + 1:
+            o.axpy_f32(d_out, g_rep, 1.0, M * D)
         g = self.buf('gx', (M, D), F32)
         o.rmsnorm_bwd(d_out, st['x_last'], self.P('transformer.norm.gamma'), g, self.G('transformer.norm.gamma'), M, D)
 
@@ -835,6 +865,8 @@ class Engine:
               (o.attn_residual_bwd_h16 if self.hid_bf16 else o.attn_residual_bwd)(self._ptr_array(hid[:i + 2]), self._ptr_array(dH[:i + 2]), i + 2, self.P(f'{pre}.3.norm_keys.gamma'), self.P(f'{pre}.3.pseudo_queries'),
                                 g, L['xr'], L['rlse'], self.G(f'{pre}.3.norm_keys.gamma'), self.G(f'{pre}.3.pseudo_queries'), arws, M, D, 1 if i == self.depth - 1 else 0)
             gx = dH[i + 1]                       # complete gradient w.r.t. x_c of this layer; updated in place below
+            if rep_at == i + 1:
+                o.axpy_f32(gx, g_rep, 1.0, M * D)
             # -- feed-forward branch
             o.resid_bwd(gx, L['yF'], cond_row, st['zg'][:, wF * D:] if nc > 0 else None, zg_ld, self.P(f'{pre}.2.layerscale'), dy,
                         dzg[:, wF * D:] if nc > 0 else None, zg_ld, self.G(f'{pre}.2.layerscale'), self.G(f'{pre}.2.fn.net.3.bias'), M, D)
@@ -919,6 +951,8 @@ class Engine:
             o.attn_residual_bwd2(self._ptr_array(hid[:1]), 1, 0, self._ptr_array(gam), self._ptr_array(pqs), self._ptr_array([dxs[j] for j in allj]),
                                  self._ptr_array([arsc[j][0, 0] for j in allj]), len(allj), None, None, None, dH[0], None, sc_stride, None, None, None, M, D)
         o.axpy_f32(g, dH[0], 1.0, M * D)
+        if rep_at == 0:
+            o.axpy_f32(g, g_rep, 1.0, M * D)
         dmodtok = self.buf('dmodtok', (max(S, 1), D), BF16)
         o.embed_bwd(g, dv['text_id'], dv['slot'] if S > 0 else None, self.G('text_embed.weight'), dmodtok if S > 0 else None, M, D)
         if S > 0:
@@ -1007,3 +1041,90 @@ class Engine:
                            self.opt_step, grad_scale, int(zero_grads), step_dev)
         self._grads_clean = bool(zero_grads)
         self._dirty = True
+
+
+class RepHead:
+    """Self-Flow predictor head and representation loss (`SelfMaskedRepTraining`, T.py:3490-3493, 3455-3460, 3556-3559) on the kernels of the
+    block stack, in the student engine's workspaces:  u = RMSNorm(x) (final-norm row kernel) -> GEGLU GEMM epilogue -> a = W2 h + b2 ->
+    loss = 1 - mean cos(a, teacher rows) with da in the same pass (tfx_rep_cos_fwd_bwd).  `head` is `Sequential(RMSNorm, FeedForward)` with the
+    reference's parameter names (`0.gamma`, `1.net.0.*`, `1.net.3.*`); its gradients accumulate into the parameters' `.grad`."""
+
+    def __init__(self, engine: Engine, head):
+        self.eng, self.head = engine, head
+        self._ptrs = None
+
+    def _prepare(self):
+        head, dev = self.head, self.eng.device
+        gamma, w1, b1, w2, b2 = head[0].gamma, head[1].net[0].weight, head[1].net[0].bias, head[1].net[3].weight, head[1].net[3].bias
+        ptrs = tuple(p.data_ptr() for p in (gamma, w1, b1, w2, b2))
+        if ptrs != self._ptrs:
+            D, inner = w1.shape[1], w2.shape[1]
+            Ip = _round_up(inner, 64)
+            assert w1.is_cuda and all(p.dtype == F32 and p.is_contiguous() for p in (gamma, w1, b1, w2, b2)), 'the predictor head must hold contiguous fp32 cuda parameters'
+            src = w1_row_src(inner)
+            src32 = torch.from_numpy(src.astype(np.int32)).to(dev)
+            self.w1p = torch.zeros(2 * Ip, D, device = dev, dtype = BF16)
+            self.w2p = torch.zeros(D, Ip, device = dev, dtype = BF16)
+            self.b1p = torch.zeros(2 * Ip, device = dev, dtype = F32)
+            jobs = [(w1, D, D, src32, self.w1p, 2 * Ip, D, 0), (w2, inner, inner, None, self.w2p, D, Ip, 0), (b1, 1, 1, src32, self.b1p, 2 * Ip, 1, 1)]
+            self.pack = pack_job_table(jobs, dev)
+            self.b1_cols = src32
+            self.w1_rows = torch.from_numpy(np.where(src >= 0, src * D, -1)).to(dev)
+            self.w2_rows = torch.from_numpy(np.arange(D, dtype = np.int64) * inner).to(dev)
+            self.D, self.inner, self.Ip, self._ptrs = D, inner, Ip, ptrs
+        return gamma, b2
+
+    def forward(self, x: Tensor, teacher: Tensor, g: Tensor) -> Tensor:
+        """x: fp32 [M, D] student rows; teacher: bf16 / fp32 [M, D] rows; g: fp32 [1] device scalar d(total)/d(loss) the gradient is computed
+        for.  Returns the loss (fp32 device scalar, mean over the M rows)."""
+        eng, o = self.eng, self.eng.ops
+        gamma, b2 = self._prepare()
+        M, D, Ip = x.shape[0], self.D, self.Ip
+        assert x.dtype == F32 and x.shape == teacher.shape == (M, D) and teacher.dtype in (F32, BF16) and x.is_contiguous() and teacher.is_contiguous()
+        o.cast_pack_multi(*self.pack)
+        u = eng.buf('rh_u', (M, D), BF16)
+        o.rmsnorm_fwd(x, gamma, None, u, None, None, M, D)
+        vg = eng.buf('rh_vg', (M, 2 * Ip), BF16); h = eng.buf('rh_h', (M, Ip), BF16)
+        o.gemm_geglu(u, D, self.w1p, D, self.b1p, M, 2 * Ip, D, vg, h)
+        a = eng.buf('rh_a', (M, D), F32)
+        o.gemm_store(h, Ip, 0, self.w2p, Ip, 0, M, D, Ip, a, D, None, 0, b2, None, 1.0, 0, 1)
+        da = eng.buf('rh_da', (M, D), BF16)
+        part = eng.buf('rh_part', (int(o.lib.tfx_rep_cos_blocks(M)),), torch.float64)
+        ticket = eng.buf('rh_ticket', (1,), I32, zero = True)
+        loss = eng.buf('rh_loss', (1,), F32)
+        o.rep_cos_fwd_bwd(a, teacher, 1 if teacher.dtype == BF16 else 0, g, M, da, part, ticket, loss, M, D)
+        self.state = dict(x = x, u = u, vg = vg, h = h, da = da, g = g, M = M)
+        return loss[0].clone()
+
+    def backward(self, g_loss: Tensor | None = None) -> Tensor:
+        """Accumulates the head's parameter gradients; returns d(total)/dx (fp32 [M, D], an engine workspace).  `g_loss`: autograd's
+        d(total)/d(loss) when it differs from the forward's `g` (da is rescaled by g_loss / g)."""
+        eng, o, st = self.eng, self.eng.ops, self.state
+        M, D, inner, Ip = st['M'], self.D, self.inner, self.Ip
+        head = self.head
+        params = [head[0].gamma, head[1].net[0].weight, head[1].net[0].bias, head[1].net[3].weight, head[1].net[3].bias]
+        for p in params:
+            if p.grad is None:
+                p.grad = torch.zeros_like(p)
+        ggamma, gw1, gb1, gw2, gb2 = (p.grad for p in params)
+        da = st['da']
+        if g_loss is not None:
+            o.scale_bf16(da, (g_loss.detach().float().reshape(1) / st['g']), da.numel())
+        sms = torch.cuda.get_device_properties(eng.device).multi_processor_count
+        ks = max(1, min(64, M // 2048))
+        dh = eng.buf('rh_dh', (M, Ip), BF16)
+        o.gemm_store(da, D, 0, self.w2p, Ip, 1, M, Ip, D, None, 0, dh, Ip, None, None, 1.0, 0, 1)
+        o.gemm_store(da, D, 1, st['h'], Ip, 1, D, inner, M, gw2, 0, None, 0, None, self.w2_rows, 1.0, 1, wgrad_splits(D, inner, M, sms, ks))
+        o.colsum_bf16(da, D, M, D, None, gb2)
+        dvg = eng.buf('rh_dvg', (M, 2 * Ip), BF16)
+        rpb = o.lib.tfx_geglu_bwd_rows_per_block()
+        nblk = (M + rpb - 1) // rpb
+        part = eng.buf('rh_geglu_part', (nblk, 2 * Ip), F32)
+        o.geglu_bwd(dh, st['vg'], dvg, M, Ip, None, None, part)
+        o.colsum_f32(part, 2 * Ip, nblk, 2 * Ip, self.b1_cols, gb1)
+        du = eng.buf('rh_du', (M, D), F32)
+        o.gemm_store(dvg, 2 * Ip, 0, self.w1p, D, 1, M, D, 2 * Ip, du, D, None, 0, None, None, 1.0, 0, 1)
+        o.gemm_store(dvg, 2 * Ip, 1, st['u'], D, 1, 2 * Ip, D, M, gw1, 0, None, 0, None, self.w1_rows, 1.0, 1, wgrad_splits(2 * Ip, D, M, sms, ks))
+        gx = eng.buf('rh_gx', (M, D), F32)
+        o.rmsnorm_bwd(du, st['x'], head[0].gamma, gx, ggamma, M, D)
+        return gx

@@ -178,7 +178,13 @@ def pack_batch(
     return_loss: bool,
     return_embed: bool,
     need_axial_pos_emb: bool = False,
+    pad_rows: bool = False,
 ) -> RaggedBatch:
+    """`pad_rows` (training batches): every sample is fed at the length of the longest, as in the reference's padded `[b, n]` layout
+    (MP.py:573 pads with -1, T.py:3136-3144 shifts, T.py:3173 embeds -1 as token 0).  A shorter sample's pad positions are its last token,
+    which the shift no longer cuts, then token 0: text rows with label -1, causal attention (they see their sample, no real row sees them) and
+    continuing rotary positions.  They change no loss term (`total_tokens` and `n_valid` count the real tokens only); the Self-Flow
+    representation loss averages over them as the reference does."""
     B = len(modalities)
     n_types = model.num_modalities
     times_np = None
@@ -235,6 +241,15 @@ def pack_batch(
         full_lens.append(offset); modality_positions.append(positions)
     sample_piece0.append(len(pieces))
 
+    total_tokens = sum(full_lens)
+    if pad_rows and return_loss and B and min(full_lens) < max(full_lens):
+        L, padded, p0 = max(full_lens), [], []
+        for b in range(B):
+            p0.append(len(padded))
+            padded += [(p, i) for p, i in zip(pieces[sample_piece0[b]:sample_piece0[b + 1]], piece_inst[sample_piece0[b]:sample_piece0[b + 1]])]
+            padded.append((_neg_ids(L - full_lens[b]), -1))
+        pieces, piece_inst = [p for p, _ in padded], [i for _, i in padded]
+        sample_piece0, full_lens = p0 + [len(padded)], [L] * B
     full_lens = np.asarray(full_lens, dtype = np.int64)
     drop = 1 if return_loss else 0
     seq_lens = np.maximum(full_lens - drop, 0)
@@ -322,7 +337,7 @@ def pack_batch(
         cond_times = np.asarray(cond_times, dtype = np.float32), n_types = n_types,
         type_rows = [(int(type_base[t]), int(type_base[t + 1])) for t in range(n_types)], row_token = row_token, row_time = row_time,
         latents = latents, instances = instances, modality_positions = modality_positions,
-        total_tokens = int(full_lens.sum()), n_type_tokens = n_type_tokens, max_rope_pos = max_rope, has_labels = return_loss)
+        total_tokens = int(total_tokens), n_type_tokens = n_type_tokens, max_rope_pos = max_rope, has_labels = return_loss)
     rb.n_valid = int((label >= 0).sum())
     add_pos = getattr(model, 'add_pos_emb', None)
     if add_pos is not None and any(add_pos) and instances:
@@ -428,8 +443,9 @@ def pack_text_only(text: Tensor, *, return_loss: bool, pos_offset: int = 0) -> R
 
 # --------------------------------------------------------------------------------------------- registry (API parity)
 def _strategy(name):
-    def fn(modalities, times, model, *, need_axial_pos_emb, return_loss, return_embed):
-        return pack_batch(modalities, times, model, return_loss = return_loss, return_embed = return_embed, need_axial_pos_emb = need_axial_pos_emb)
+    def fn(modalities, times, model, *, need_axial_pos_emb, return_loss, return_embed, pad_rows = False):
+        return pack_batch(modalities, times, model, return_loss = return_loss, return_embed = return_embed, need_axial_pos_emb = need_axial_pos_emb,
+                          pad_rows = pad_rows)
     fn.__name__ = f'process_modality_batch_{name}'
     return fn
 

@@ -7,12 +7,14 @@ versa.  What differs is everything underneath: the modules below only OWN parame
 the block stack, attention, loss heads and optimizer runs in the sm_90a kernels of `libtfx_b200.so`
 driven by `engine.Engine` over the ragged descriptor of `modality_processing.pack_batch`.
 
-Out of scope here (raise loudly): U-Net pre/post encoders (`pre_post_transformer_enc_dec`), attention dropout, dim_head != 64.
+Out of scope here (raise loudly): U-Net pre/post encoders (`pre_post_transformer_enc_dec`), attention dropout, dim_head != 64, a custom
+`loss_fn` of `SelfMaskedRepTraining`.
 """
 from __future__ import annotations
 
 import math
 from functools import partial
+from itertools import chain
 from typing import Callable, NamedTuple
 
 import numpy as np
@@ -238,7 +240,8 @@ class Transformer(Module):
 
     def ff_dropout_p(self, train: bool, training: bool) -> float:
         """FFN dropout probability of one forward: nn.Dropout drops only in training mode (`training`, of the owning Transfusion), and only a
-        forward that keeps its activations for a backward (`train`) is a training forward; sampling, eval and the EMA teacher never drop."""
+        forward that keeps its activations for a backward (`train`) is a training forward; sampling, eval and the velocity-consistency EMA model
+        never drop.  The Self-Flow teacher's inference forward (`SelfMaskedRepTraining`) passes train = True here: in training mode it drops."""
         return self.ff_dropout if (train and training) else 0.
 
     def forward(self, *args, **kwargs):
@@ -256,11 +259,14 @@ class _TrainStep(torch.autograd.Function):
         ctx.engine = engine
         engine._last_vel = res.get('vel')
         engine._last_res = res
+        if 'rep' in res:            # a hidden state handed out in packed rows (`rep_layer`): its gradient comes back to backward()
+            return res['total'], res['text'], res['flows'], res['rep']
         return res['total'], res['text'], res['flows']
 
     @staticmethod
-    def backward(ctx, g_total, g_text, g_flows):
-        ctx.engine.backward(gscale = g_total, bucket_cb = getattr(ctx.engine, '_bucket_cb', None))
+    def backward(ctx, g_total, g_text, g_flows, *g_rep):
+        kw = dict(g_rep = g_rep[0]) if g_rep else {}
+        ctx.engine.backward(gscale = g_total, bucket_cb = getattr(ctx.engine, '_bucket_cb', None), **kw)
         return None, None, None, None, None, None
 
 
@@ -486,9 +492,12 @@ class Transfusion(SamplingMixin, Module):
             kw.setdefault('recon_weight', self.reconstruction_loss_weight)
         if train and torch.is_grad_enabled():
             anchor = self.text_embed.weight
-            total, text, flows = _TrainStep.apply(eng, rb, latents, eps, kw, anchor)
+            total, text, flows, *rep = _TrainStep.apply(eng, rb, latents, eps, kw, anchor)
             last = eng._last_res
-            return dict(total = total, text = text, flows = flows, vel = eng._last_vel, recon = last.get('recon'), recon_inst = last.get('recon_inst'), preds = last.get('preds'))
+            out = dict(total = total, text = text, flows = flows, vel = eng._last_vel, recon = last.get('recon'), recon_inst = last.get('recon_inst'), preds = last.get('preds'))
+            if rep:
+                out['rep'] = rep[0]
+            return out
         return eng.forward(rb, latents, eps, train = train, **kw)
 
     def _recon_breakdown(self, rb, res):
@@ -691,10 +700,12 @@ class Transfusion(SamplingMixin, Module):
         return t.reshape(-1, self.dim_latents[mt]).float().to(self.device).clone()
 
     # ------------------------------------------------------------------ host side of forward(): CFG dropout, encoders, times, pack / route
-    def pack(self, modalities, times = None, num_modalities_to_times_fn = None, prob_uncond = None, return_loss = True, return_embed = False, is_decoding = False):
+    def pack(self, modalities, times = None, num_modalities_to_times_fn = None, prob_uncond = None, return_loss = True, return_embed = False, is_decoding = False,
+             pad_rows = False):
         """Everything `forward` does on the host before the first kernel (transfusion.py:3011-3082 + modality_processing): returns the ragged
         batch descriptor and the times that were used.  Exposed so that a training loop can pack step i+1 while step i runs on the device
-        (`DataParallelTrainer` does, and replays a captured CUDA graph when the descriptor has the same shape signature)."""
+        (`DataParallelTrainer` does, and replays a captured CUDA graph when the descriptor has the same shape signature).
+        `pad_rows`: feed every sample at the longest sample's length (`modality_processing.pack_batch`), as `SelfMaskedRepTraining` does."""
         batch = len(modalities)
         samples = [list(s) if isinstance(s, list) else s for s in modalities]
         if return_loss:
@@ -729,7 +740,7 @@ class Transfusion(SamplingMixin, Module):
             fn = default(num_modalities_to_times_fn, default_modality_length_to_time_fn)
             times = fn(tensor(n_mods))
         process = get_processing_strategy(self.modality_processing)
-        rb = process(samples, times, self, need_axial_pos_emb = any(self.add_pos_emb), return_loss = return_loss, return_embed = return_embed)
+        rb = process(samples, times, self, need_axial_pos_emb = any(self.add_pos_emb), return_loss = return_loss, return_embed = return_embed, pad_rows = pad_rows)
         return rb, times
 
     # ------------------------------------------------------------------ main forward (transfusion.py:2925-3450)
@@ -839,3 +850,112 @@ class Transfusion(SamplingMixin, Module):
         if return_times:
             ret = (*ret, times)
         return ret[0] if len(ret) == 1 else ret
+
+
+# ------------------------------------------------------------------------------------------- Self-Flow (T.py:3452-3569)
+def default_rep_loss_fn(pred, target):
+    """1 - mean cosine similarity over the last dim (T.py:3458-3460); `SelfMaskedRepTraining` runs it as the fused tfx_rep_cos_fwd_bwd kernel"""
+    return 1. - torch.nn.functional.cosine_similarity(pred, target, dim = -1).mean()
+
+
+class _RepLoss(torch.autograd.Function):
+    """The predictor head and the representation loss as one node: its backward runs before the student's (`rep` is a `_TrainStep` output), so
+    the engine's backward receives the gradient of the student's hidden state."""
+
+    @staticmethod
+    def forward(ctx, head, rep, teacher_rep, g, anchor):
+        ctx.head = head
+        return head.forward(rep, teacher_rep, g)
+
+    @staticmethod
+    def backward(ctx, g_loss):
+        return None, ctx.head.backward(g_loss), None, None, None
+
+
+class SelfMaskedRepTraining(Module):
+    """Self-Flow training (T.py:3452-3569): the student's hidden state at `student_layer`, through a predictor head (RMSNorm + GEGLU FeedForward),
+    is pulled towards the EMA teacher's hidden state at `teacher_layer` by 1 - mean cosine similarity, averaged over the padded [b, n] layout as
+    in the reference (pad rows: `modality_processing.pack_batch`).  Asymmetric dropout sets the student's and the teacher's FFN dropout (the
+    `nn.Dropout` modules `set_dropout_` reaches); attention dropout exists only as the no-op of `use_flex_attn`.  The teacher is an inference
+    forward of the EMA engine that keeps its hidden states; the head runs on the block stack's kernels (`engine.RepHead`)."""
+
+    def __init__(self, net: Transfusion, ema_beta = 0.999, rep_loss_weight = 0.1, student_layer = -3, teacher_layer = -1, loss_fn = default_rep_loss_fn,
+                 use_asymmetric_dropout = True, student_dropout_rate = 0.1, teacher_dropout_rate = 0.):
+        super().__init__()
+        assert not use_asymmetric_dropout or student_dropout_rate > teacher_dropout_rate, 'student must have greater dropout rate than teacher to ensure teacher has a better view'
+        if loss_fn is not default_rep_loss_fn:
+            raise NotImplementedError('loss_fn: only the default (1 - mean cosine similarity) is implemented, as the fused kernel tfx_rep_cos_fwd_bwd')
+        if use_asymmetric_dropout and (student_dropout_rate or teacher_dropout_rate) and not net.transformer.use_flex_attn:
+            raise NotImplementedError('asymmetric dropout sets attention dropout, which the attention kernels do not implement; '
+                                      'only use_flex_attn = True (no attention dropout in the reference either) is supported')
+        n_hid = net.transformer.depth + 2
+        for name, layer in (('student_layer', student_layer), ('teacher_layer', teacher_layer)):
+            if not -n_hid <= layer < n_hid:
+                raise IndexError(f'{name} = {layer}: the hidden states are [tokens, layer 1 .. {n_hid - 2}, final norm] ({n_hid} entries)')
+        self.student = net
+        self.teacher = net.create_ema(beta = ema_beta)
+        self.rep_loss_weight = rep_loss_weight
+        self.has_ssl_loss = rep_loss_weight > 0
+        self.use_asymmetric_dropout = use_asymmetric_dropout
+        self.student_dropout_rate, self.teacher_dropout_rate = student_dropout_rate, teacher_dropout_rate
+        self.student_layer, self.teacher_layer = student_layer, teacher_layer
+        self.loss_fn = loss_fn
+        dim = net.dim
+        self.student_predict_head = nn.Sequential(_Gamma(dim), _FeedForwardParams(dim, int(dim * 4 * 2 / 3)))      # RMSNorm(dim), FeedForward(dim)
+        self.register_buffer('zero', tensor(0.))
+        self.teacher.ema_model.train(self.training)        # a registered sub-module: the teacher follows the wrapper's .train() / .eval()
+        self._head = None
+
+    def parameters(self):
+        return chain(self.student.parameters(), self.student_predict_head.parameters())
+
+    def update_teacher(self):
+        self.teacher.update()
+
+    def forward(self, modalities, times = None, num_modalities_to_times_fn = None, prob_uncond = None, noise = None, teacher_noise = None, dropout_key = None):
+        """Returns total, (student loss, Self-Flow loss).  `modalities`: interleaved samples (the only input the reference wrapper takes: its tensor
+        forwards return no times).  `noise` / `teacher_noise`: per type [S_t, dim_latent] flow noise of the student's / the teacher's forward, as
+        `Transfusion.forward(noise = ...)`; `dropout_key`: the student's FFN dropout masks (the teacher draws its own)."""
+        if is_tensor(modalities):
+            raise TypeError('SelfMaskedRepTraining takes interleaved sample lists (the reference wrapper needs the times of that forward)')
+        student, ema = self.student, self.teacher
+        if self.use_asymmetric_dropout:                    # set_dropout_ (T.py:156-159), persisting on the student
+            student.transformer.ff_dropout = float(self.student_dropout_rate)
+        if not self.has_ssl_loss:
+            loss = student(modalities, times = times, num_modalities_to_times_fn = num_modalities_to_times_fn, prob_uncond = prob_uncond, noise = noise,
+                           dropout_key = dropout_key)
+            return loss, (loss, self.zero)
+        n_hid = student.transformer.depth + 2
+
+        def run(model, times_, noise_):
+            rb, used_times = model.pack(modalities, times = times_, num_modalities_to_times_fn = num_modalities_to_times_fn, prob_uncond = prob_uncond,
+                                        return_loss = True, pad_rows = True)
+            lat = model._latents_to_device(rb)
+            if exists(noise_):
+                eps = [n.reshape(-1, model.dim_latents[t]).float().to(model.device) if exists(n) else None for t, n in enumerate(noise_)]
+            else:
+                eps = [torch.randn_like(l) if exists(l) else None for l in lat]
+            return rb, used_times, lat, eps
+
+        rb, times_used, lat, eps = run(student, times, noise)
+        res = student._run(rb, lat, eps, train = True, text_loss_weight = student.text_loss_weight, flow_loss_weight = student.flow_loss_weight,
+                           dropout_key = dropout_key, rep_layer = self.student_layer % n_hid)
+        student._last_batch = rb
+        student_loss = res['total']
+
+        teacher = ema.ema_model
+        ema._engines()
+        if self.use_asymmetric_dropout:
+            teacher.transformer.ff_dropout = float(self.teacher_dropout_rate)
+        with torch.no_grad():
+            rb_t, _, lat_t, eps_t = run(teacher, times_used, teacher_noise)          # the student's times (T.py:3539)
+            assert rb_t.M == rb.M
+            dropout = teacher.transformer.ff_dropout_p(True, teacher.training) > 0.
+            tres = teacher.engine.forward(rb_t, lat_t, eps_t, train = False, want_logits = False, want_preds = False, rep_layer = self.teacher_layer % n_hid,
+                                          dropout = dropout)
+        if self._head is None or self._head.eng is not student.engine:
+            from .engine import RepHead
+            self._head = RepHead(student.engine, self.student_predict_head)
+        g = torch.full((1,), float(self.rep_loss_weight), device = student.engine.device)        # d total / d loss of a plain total.backward()
+        ssl = _RepLoss.apply(self._head, res['rep'], tres['rep'], g, self.student_predict_head[0].gamma)
+        return student_loss + ssl * self.rep_loss_weight, (student_loss, ssl)
