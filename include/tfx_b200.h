@@ -33,6 +33,15 @@ int tfx_init(int device);                       /* checks the device is sm_90 */
  * the environment (TFX_GEMM_CLUSTER).  No reference counterpart: a tuning knob of this library.   */
 int tfx_gemm_set_cluster_mode(int mode);
 
+/* Tile of tfx_gemm_store: 1 = 256 x 128 cooperative tile for launches with at least 16 k-blocks (K / 64 / splits) per work item and CTA pairing
+ * off, else 128 x 128 ping-pong (default); 2 = always the 256 x 128 tile; 3 = never.  Both compute bit-identical outputs; this is for tests and
+ * benchmarks that compare them.  No reference counterpart. */
+int tfx_gemm_set_wide_mode(int mode);
+
+/* Launch geometry tfx_gemm_store would use for these arguments under the current modes: geometry[0] work items (tiles x splits),
+ * [1] k-blocks (64 deep) per item, [2] tile rows (128 or 256), [3] split-K factor after clamping.  Launches nothing.  No reference counterpart. */
+int tfx_gemm_store_items(int M, int N, int K, int a_mn_major, int b_mn_major, int k_splits, int* geometry);
+
 /* generic: out = alpha*acc + bias[n]  -> fp32 (store / atomic accumulate, optional per-row offsets) and/or bf16.
  * Replaces nn.Linear call sites with no fused tail: to_time_cond Linear (T.py:1070,1132), to_film /
  * to_ada_ln_zero evaluated per distinct time (T.py:700,712,749,767), to_text_logits (T.py:3280,2640),

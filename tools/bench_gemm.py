@@ -13,6 +13,8 @@ if os.environ.get('TFX_LIB'):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--dump', default = None, metavar = 'DIR', help = 'write the outputs of every non-split-K case to DIR/*.npy')
+    ap.add_argument('--tiles', action = 'store_true', help = 'the plain-store (dgrad / wgrad) shapes of the train step with the 256 x 128 '
+                    'cooperative tile and the 128 x 128 ping-pong tile alternated (tfx_gemm_set_wide_mode); with --dump both outputs per case')
     args = ap.parse_args()
     ops = _lib.Ops()
     M, D, Ip, H = int(os.environ.get('TOKENS', 131072)), 512, 1408, 8
@@ -64,6 +66,8 @@ def main():
     tag = os.path.basename(os.environ.get('TFX_LIB', 'default'))
     if args.dump:
         os.makedirs(args.dump, exist_ok = True)
+    if args.tiles:
+        return compare_tiles(ops, M, D, Ip, big, args.dump)
     for name, (fn, fl, outs) in cases.items():
         for _ in range(3): fn()
         ts = []
@@ -79,5 +83,54 @@ def main():
             for tn, t in outs.items():
                 a = t.cpu()
                 np.save(os.path.join(args.dump, f'{case}.{tn}.npy'), (a.view(torch.int16) if a.dtype == bf else a).numpy())
+def compare_tiles(ops, M, D, Ip, big, dump):
+    """tfx_gemm_store at the train step's long-K shapes (and two short-K ones) with each tile; the wgrads use the split count the engine picks
+    (`engine.wgrad_splits`, default mode) for both tiles and write rows of the flat gradient buffer as the engine does (the [512 x 1365] rows
+    start 1365 floats apart, so three in four are not 16-byte aligned)"""
+    from transfusion_pytorch_b200.engine import wgrad_splits
+    bf = torch.bfloat16
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    g = torch.Generator(device = 'cuda').manual_seed(1)
+    r = lambda *s: (torch.randn(*s, device = 'cuda', generator = g) * 0.05).to(bf)
+    NQ, inner = 3 * 8 * 64 + 128, 1365
+    cases = {}      # name: (launch, algorithmic FLOPs, output, split-K)
+    def dgrad(N, K):
+        a, b, out = r(M, K), r(K, N), torch.empty(M, N, device = 'cuda', dtype = bf)      # dY [M, K] x W stored [K][N] (MN-major)
+        cases[f'dgrad [{M} x {N} x {K}]'] = (lambda: ops.gemm_store(a, K, 0, b, N, 1, M, N, K, None, 0, out, N, None, None, 1.0, 0, 1), 2.0 * M * N * K, out, 1)
+    def wgrad(n_out, n_in):
+        s = wgrad_splits(n_out, n_in, M, sms)
+        a, b = r(M, n_out), r(M, (n_in + 63) // 64 * 64)
+        flat = torch.zeros(n_out * n_in + 4, device = 'cuda')
+        rows = torch.arange(n_out, device = 'cuda', dtype = torch.int64) * n_in + 4    # offset 4: the first row aligned, as no real one needs to be
+        cases[f'wgrad [{n_out} x {n_in} x {M}] splits {s}'] = (lambda: ops.gemm_store(a, n_out, 1, b, b.shape[1], 1, n_out, n_in, M, flat, 0, None, 0, None, rows,
+                                                                                     1.0, 1, s), 2.0 * M * n_out * n_in, flat, s)
+    dgrad(D, 2 * Ip); wgrad(2 * Ip, D); wgrad(D, inner); dgrad(D, NQ); wgrad(NQ, D); wgrad(D, D); dgrad(2 * Ip // 2, D); dgrad(D, D)
+    modes = {'wide': 2, 'pingpong': 3}
+    for name, (fn, fl, out, s) in cases.items():
+        res, ts = {}, {m: [] for m in modes}
+        for m, code in modes.items():                       # warm-up, and the output of each tile from a zeroed destination
+            ops.lib.tfx_gemm_set_wide_mode(code)
+            out.zero_(); fn(); torch.cuda.synchronize()
+            res[m] = out.clone()
+            for _ in range(2): fn()
+        for _ in range(10):
+            for m, code in modes.items():
+                ops.lib.tfx_gemm_set_wide_mode(code)
+                big.zero_()                                 # flush L2
+                e0, e1 = torch.cuda.Event(enable_timing = True), torch.cuda.Event(enable_timing = True)
+                e0.record(); fn(); e1.record(); torch.cuda.synchronize()
+                ts[m].append(e0.elapsed_time(e1) * 1e3)
+        ops.lib.tfx_gemm_set_wide_mode(1)
+        med = {m: sorted(t)[5] for m, t in ts.items()}
+        same = 'bit-identical' if torch.equal(res['wide'], res['pingpong']) else f'max |diff| {(res["wide"].float() - res["pingpong"].float()).abs().max().item():.3g}'
+        print(f'{name:44s} ' + '  '.join(f'{m} {med[m]:7.1f} us ({fl / med[m] / 1e6:5.1f} TFLOP/s)' for m in modes)
+              + f'  wide/pingpong {med["wide"] / med["pingpong"]:.3f}  outputs {same}' + (' (split-K atomics)' if s > 1 else ''), flush = True)
+        if dump:
+            case = name.split()[0] + '_' + name.split('[')[1].split(']')[0].replace(' x ', 'x')
+            for m, t in res.items():
+                a = t.cpu()
+                np.save(os.path.join(dump, f'{case}.{m}.npy'), (a.view(torch.int16) if a.dtype == bf else a).numpy())
+
+
 if __name__ == '__main__':
     main()

@@ -20,6 +20,8 @@ VP, I, LL, F, ULL = c_void_p, c_int, c_longlong, c_float, c_ulonglong
 SIGNATURES = {
     'tfx_init': [I],
     'tfx_gemm_set_cluster_mode': [I],
+    'tfx_gemm_set_wide_mode': [I],
+    'tfx_gemm_store_items': [I, I, I, I, I, I, VP],
     'tfx_gemm_store': [VP, LL, I, VP, LL, I, I, I, I, VP, LL, VP, LL, VP, VP, F, I, I, VP],
     'tfx_gemm_qkvg': [VP, LL, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP],
     'tfx_gemm_resid': [VP, LL, VP, LL, I, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, VP, LL, VP, VP],
@@ -126,6 +128,14 @@ def check(rc: int, name: str):
     if rc != 0:
         msg = _lib.tfx_last_error().decode(errors = 'replace') if _lib is not None else ''
         raise TfxError(f'{name} failed (code {rc}): {msg}')
+
+
+def gemm_store_items(M: int, N: int, K: int, a_mn: int, b_mn: int, k_splits: int):
+    """(work items, k-blocks per item, tile rows, split-K factor) of a `tfx_gemm_store` launch with these arguments; launches nothing"""
+    lib = load()
+    geo = (c_int * 4)()
+    check(lib.tfx_gemm_store_items(M, N, K, a_mn, b_mn, k_splits, geo), 'tfx_gemm_store_items')
+    return tuple(geo)
 
 
 class Ops:

@@ -20,6 +20,12 @@ static int finish(int rc, const char* what) {
 
 static int dispatch_major(const GemmOperand& A, const GemmOperand& B, const GemmParams& p, cudaStream_t st) {
   const int sms = num_sms();
+  if (gemm_store_wide(p.K, p.k_splits)) {
+    if (!A.mn_major && !B.mn_major) return launch_gemm_wide_t<false, false>(A, B, p, sms, st);
+    if (!A.mn_major && B.mn_major) return launch_gemm_wide_t<false, true>(A, B, p, sms, st);
+    if (A.mn_major && B.mn_major) return launch_gemm_wide_t<true, true>(A, B, p, sms, st);
+    return launch_gemm_wide_t<true, false>(A, B, p, sms, st);
+  }
   if (!A.mn_major && !B.mn_major) return launch_gemm_t<false, false, EPI_STORE>(A, B, p, sms, st);
   if (!A.mn_major && B.mn_major) return launch_gemm_t<false, true, EPI_STORE>(A, B, p, sms, st);
   if (A.mn_major && B.mn_major) return launch_gemm_t<true, true, EPI_STORE>(A, B, p, sms, st);
@@ -31,6 +37,24 @@ extern "C" {
 int tfx_gemm_set_cluster_mode(int mode) {
   TFX_REQUIRE(mode >= 1 && mode <= 3, "gemm_set_cluster_mode: mode %d not in {1 (never pair, default), 2 (always pair), 3 (pair long-K launches)}", mode);
   gemm_cluster_mode_ref() = mode;
+  return 0;
+}
+
+int tfx_gemm_set_wide_mode(int mode) {
+  TFX_REQUIRE(mode >= 1 && mode <= 3, "gemm_set_wide_mode: mode %d not in {1 (long work items, default), 2 (always), 3 (never)}", mode);
+  gemm_wide_mode_ref() = mode;
+  return 0;
+}
+
+int tfx_gemm_store_items(int M, int N, int K, int a_mn_major, int b_mn_major, int k_splits, int* geometry) {
+  TFX_REQUIRE(M > 0 && N > 0 && K > 0 && geometry, "gemm_store_items: needs M, N, K > 0 (got %d, %d, %d) and an output array", M, N, K);
+  (void)a_mn_major; (void)b_mn_major;      // the tile does not depend on the operand layouts today
+  const int tile_m = gemm_store_wide(K, k_splits) ? GemmWideCfg::BM : GEMM_BM;
+  const int s = gemm_effective_splits(K, k_splits);
+  geometry[0] = ((M + tile_m - 1) / tile_m) * ((N + GEMM_BN - 1) / GEMM_BN) * s;
+  geometry[1] = gemm_kb_per_item(K, s);
+  geometry[2] = tile_m;
+  geometry[3] = s;
   return 0;
 }
 

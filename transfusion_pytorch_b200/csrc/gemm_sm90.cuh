@@ -230,6 +230,104 @@ __device__ __forceinline__ void stg_store_rows(const uint8_t* sw, int lane, uint
   }
 }
 
+// EPI_STORE epilogue of one 32-column slice [cbase, cbase + 32) of a warp's 32 rows: out = alpha * acc + bias.  Thread `lane` holds the
+// raw accumulators of slice row `lane` in r; slice row i is output row row_of(i).  sw is the warp's staging tile (free on entry and exit).
+// Both GEMM schedules end in this function, so their outputs agree bit for bit wherever their accumulators do.
+template <class RowOf>
+__device__ __forceinline__ void store_slice(const GemmParams& p, uint8_t* sw, int lane, uint32_t (&r)[32], int cbase, RowOf row_of) {
+  const bool f32_staged = p.out_f32 && (p.row_off || (p.ld_f32 & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_f32) & 15) == 0);
+  const bool bf16_staged = p.out_bf16 && (p.ld_bf16 & 7) == 0 && ((reinterpret_cast<uintptr_t>(p.out_bf16) & 15) == 0);
+  const int row = row_of(lane);
+  const bool row_ok = row < p.M;
+  const bool full = cbase + 32 <= p.N;
+  float v[32];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
+  if (p.alpha != 1.f) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) v[j] *= p.alpha;
+  }
+  if (p.bias) {
+    if (full) {
+#pragma unroll
+      for (int j = 0; j < 32; j += 4) { const float4 b = *reinterpret_cast<const float4*>(p.bias + cbase + j); v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w; }
+    } else {
+      for (int j = 0; j < 32; ++j) if (cbase + j < p.N) v[j] += p.bias[cbase + j];
+    }
+  }
+  if (p.out_f32) {
+    if (full && f32_staged) {
+#pragma unroll
+      for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(v[j]);
+      stg_put<8>(sw, lane, r);
+      __syncwarp();
+      auto put = [&](float* dst, float x) { if (p.accumulate_f32) atomicAdd(dst, x); else *dst = x; };
+#pragma unroll
+      for (int it = 0; it < 8; ++it) {
+        const int rr = it * 4 + (lane >> 3), ch = lane & 7;
+        const int grow = row_of(rr);
+        if (grow < p.M) {
+          const long long off = p.row_off ? p.row_off[grow] : (long long)grow * p.ld_f32;
+          if (off >= 0) {
+            float* drow = p.out_f32 + off + cbase;                  // 4-byte aligned; 16-byte aligned iff off % 4 == 0
+            const uint8_t* srow = sw + rr * 128;
+            const int a = (int)(reinterpret_cast<uintptr_t>(drow) >> 2) & 3;
+            if (a == 0) {
+              float* dst = drow + ch * 4;
+              const float4 t = *reinterpret_cast<const float4*>(srow + ((ch ^ (rr & 7)) << 4));
+              if (p.accumulate_f32) asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(t.x), "f"(t.y), "f"(t.z), "f"(t.w) : "memory");
+              else *reinterpret_cast<float4*>(dst) = t;
+            } else {
+              // a row offset that is not a multiple of 4 (the [512 x 1365] W2 gradient in the flat buffer): the first pe columns reach the next
+              // 16-byte boundary, lanes 0-6 then cover 28 columns in aligned groups of 4, and lane 7 takes the pe leading and a trailing columns
+              const int pe = 4 - a;
+              auto col = [&](int j) { return *reinterpret_cast<const float*>(srow + (((j >> 2) ^ (rr & 7)) << 4) + (j & 3) * 4); };
+              if (ch < 7) {
+                const int j = pe + 4 * ch;
+                float* dst = drow + j;
+                const float4 t = make_float4(col(j), col(j + 1), col(j + 2), col(j + 3));
+                if (p.accumulate_f32) asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(t.x), "f"(t.y), "f"(t.z), "f"(t.w) : "memory");
+                else *reinterpret_cast<float4*>(dst) = t;
+              } else {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) { const int j = i < pe ? i : 28 + i; put(drow + j, col(j)); }
+              }
+            }
+          }
+        }
+      }
+      __syncwarp();
+    } else if (row_ok) {
+      const long long off = p.row_off ? p.row_off[row] : (long long)row * p.ld_f32;
+      if (off >= 0) {
+        float* dst = p.out_f32 + off + cbase;
+        for (int j = 0; j < 32; ++j)
+          if (cbase + j < p.N) { if (p.accumulate_f32) atomicAdd(dst + j, v[j]); else dst[j] = v[j]; }
+      }
+    }
+  }
+  if (p.out_bf16) {
+    if (full && bf16_staged) {
+      uint32_t w[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) w[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
+      stg_put<4>(sw, lane, w);
+      __syncwarp();
+#pragma unroll
+      for (int it = 0; it < 4; ++it) {                           // 8 rows x 64 B per instruction
+        const int rr = it * 8 + (lane >> 2), ch = lane & 3;
+        const int grow = row_of(rr);
+        if (grow < p.M)
+          *reinterpret_cast<uint4*>(p.out_bf16 + (long long)grow * p.ld_bf16 + cbase + ch * 8) = *reinterpret_cast<const uint4*>(sw + rr * 128 + ((ch ^ (rr & 7)) << 4));
+      }
+      __syncwarp();
+    } else if (row_ok) {
+      __nv_bfloat16* dst = p.out_bf16 + (long long)row * p.ld_bf16 + cbase;
+      for (int j = 0; j < 32; ++j) if (cbase + j < p.N) dst[j] = __float2bfloat16(v[j]);
+    }
+  }
+}
+
 template <bool A_MN, bool B_MN, int EPI, int CL>
 __global__ void __launch_bounds__(384, 1)
 gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
@@ -404,78 +502,13 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if constexpr (EPI == EPI_RESID) { qk_pos = (row_ok && p.cond_row) ? p.cond_row[row] : -1; }      // (reused as the condition row)
 
       if constexpr (EPI == EPI_STORE) {
-        const bool f32_staged = p.out_f32 && (p.row_off || (p.ld_f32 & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_f32) & 15) == 0);
-        const bool bf16_staged = p.out_bf16 && (p.ld_bf16 & 7) == 0 && ((reinterpret_cast<uintptr_t>(p.out_bf16) & 15) == 0);
 #pragma unroll 1
         for (int c = 0; c < BN / 32; ++c) {
           const int cbase = col0 + c * 32;
           if (cbase >= p.N) break;
           uint32_t r[32];
           acc_ld32(acc, erow, c * 32, r);
-          const bool full = cbase + 32 <= p.N;
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-          if (p.alpha != 1.f) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] *= p.alpha;
-          }
-          if (p.bias) {
-            if (full) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) { const float4 b = *reinterpret_cast<const float4*>(p.bias + cbase + j); v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w; }
-            } else {
-              for (int j = 0; j < 32; ++j) if (cbase + j < p.N) v[j] += p.bias[cbase + j];
-            }
-          }
-          if (p.out_f32) {
-            if (full && f32_staged) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(v[j]);
-              stg_put<8>(sw, lane, r);
-              __syncwarp();
-#pragma unroll
-              for (int it = 0; it < 8; ++it) {
-                const int rr = it * 4 + (lane >> 3), ch = lane & 7;
-                if (rr < rows_valid) {
-                  const long long off = p.row_off ? p.row_off[wrow0 + rr] : (long long)(wrow0 + rr) * p.ld_f32;
-                  if (off >= 0) {
-                    float* dst = p.out_f32 + off + cbase + ch * 4;
-                    const float4 t = *reinterpret_cast<const float4*>(sw + rr * 128 + ((ch ^ (rr & 7)) << 4));
-                    if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-                      if (p.accumulate_f32) asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(t.x), "f"(t.y), "f"(t.z), "f"(t.w) : "memory");
-                      else *reinterpret_cast<float4*>(dst) = t;
-                    } else {
-                      if (p.accumulate_f32) { atomicAdd(dst, t.x); atomicAdd(dst + 1, t.y); atomicAdd(dst + 2, t.z); atomicAdd(dst + 3, t.w); }
-                      else { dst[0] = t.x; dst[1] = t.y; dst[2] = t.z; dst[3] = t.w; }
-                    }
-                  }
-                }
-              }
-              __syncwarp();
-            } else if (row_ok) {
-              const long long off = p.row_off ? p.row_off[row] : (long long)row * p.ld_f32;
-              if (off >= 0) {
-                float* dst = p.out_f32 + off + cbase;
-                for (int j = 0; j < 32; ++j)
-                  if (cbase + j < p.N) { if (p.accumulate_f32) atomicAdd(dst + j, v[j]); else dst[j] = v[j]; }
-              }
-            }
-          }
-          if (p.out_bf16) {
-            if (full && bf16_staged) {
-              uint32_t w[16];
-#pragma unroll
-              for (int j = 0; j < 16; ++j) w[j] = pack_bf16(v[2 * j], v[2 * j + 1]);
-              stg_put<4>(sw, lane, w);
-              __syncwarp();
-              stg_store<4>(sw, lane, reinterpret_cast<uint8_t*>(p.out_bf16 + (long long)wrow0 * p.ld_bf16 + cbase), p.ld_bf16 * 2, rows_valid);
-              __syncwarp();
-            } else if (row_ok) {
-              __nv_bfloat16* dst = p.out_bf16 + (long long)row * p.ld_bf16 + cbase;
-              for (int j = 0; j < 32; ++j) if (cbase + j < p.N) dst[j] = __float2bfloat16(v[j]);
-            }
-          }
+          store_slice(p, sw, lane, r, cbase, [&](int i) { return wrow0 + i; });
         }
       } else if constexpr (EPI == EPI_QKVG) {
         const int tps = p.H >> 1;             // tiles per section
@@ -681,6 +714,168 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
+// ------------------------------------------------------------------------------------------------ EPI_STORE, 256 x 128 cooperative tile
+// For plain-store launches with long work items (the dgrad / wgrad products), where the main loop is the whole cost and the ping-pong
+// epilogue overlap buys little.  Both consumer warpgroups work on ONE 256 x 128 tile: warpgroup cw owns rows 128 cw .. + 127 and issues
+// exactly the two wgmma.m64n128k16 per 16-deep k step of the ping-pong kernel, from its half of the 256-row A tile and the shared B tile,
+// so its accumulators are bit-identical to those of the 128 x 128 tile 2 m + cw there.  Per byte fetched from L2 a stage carries 4/3 of the
+// MMA work, and the same ring depth covers twice the MMA time.  A ring slot is released when all 8 consumer warps have arrived; the
+// warpgroups may drift apart by less than STAGES k-blocks, which keeps the parity waits exact.
+// No fp32 accumulator tile: after the main loop each warp moves its fragments 32 columns at a time through its own 4 KB staging tile into
+// the per-row layout of store_slice (warp q of warpgroup cw: slice rows 0-15 = tile rows 128 cw + 16 q + i, 16-31 = those + 64).
+struct GemmWideCfg {
+  static constexpr int BM = 256;
+  static constexpr int THREADS = 384;
+  static constexpr int STAGES = 4;
+  static constexpr int A_BYTES = BM * GEMM_BK * 2;
+  static constexpr int B_BYTES = GEMM_BN * GEMM_BK * 2;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;             // 48 KB
+  static constexpr int STAGING = 8 * 4096;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one block");
+};
+
+template <bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(384, 1)
+gemm_sm90_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  using Cfg = GemmWideCfg;
+  constexpr int BM = Cfg::BM, BN = GEMM_BN, STAGES = Cfg::STAGES;
+  static_assert(Cfg::STAGE_BYTES % 1024 == 0, "stage alignment");
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = smem_raw;
+  if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();
+  uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING);    // [STAGES]
+  uint64_t* empty_bar = full_bar + STAGES;                                     // [STAGES]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m_tiles = (p.M + BM - 1) / BM;
+  const int n_tiles = (p.N + BN - 1) / BN;
+  const int kb_total = (p.K + GEMM_BK - 1) / GEMM_BK;
+  const int kb_per_split = (kb_total + p.k_splits - 1) / p.k_splits;
+  const int tiles = m_tiles * n_tiles;
+  const int num_items = tiles * p.k_splits;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }    // empty: one arrival per consumer warp
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ===================================================== TMA producer
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int stage = 0; uint32_t phase = 0;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+        const int split = item / tiles;
+        const int rem = item - split * tiles;
+        const int m_blk = rem / n_tiles, n_blk = rem - m_blk * n_tiles;
+        const int kb0 = split * kb_per_split;
+        const int kb1 = min(kb0 + kb_per_split, kb_total);
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
+          uint8_t* sB = sA + Cfg::A_BYTES;
+          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+          if (!A_MN) {
+            tma_load_2d(&tmA, &full_bar[stage], sA, kb * GEMM_BK, m_blk * BM);           // one 64 x 256 box
+          } else {
+#pragma unroll
+            for (int a = 0; a < BM / 64; ++a)
+              tma_load_2d(&tmA, &full_bar[stage], sA + a * (GEMM_BK * 128), m_blk * BM + a * 64, kb * GEMM_BK);
+          }
+          if (!B_MN) {
+            tma_load_2d(&tmB, &full_bar[stage], sB, kb * GEMM_BK, n_blk * BN);
+          } else {
+#pragma unroll
+            for (int a = 0; a < BN / 64; ++a)
+              tma_load_2d(&tmB, &full_bar[stage], sB + a * (GEMM_BK * 128), n_blk * BN + a * 64, kb * GEMM_BK);
+          }
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================================================== consumers: both warpgroups on every item
+    setmaxnreg_inc<232>();
+    const int cw = (warp >> 2) - 1;            // rows 128 cw .. + 127 of the tile
+    const int quad = warp & 3;                 // fragment rows 16 quad .. + 15 of each 64-row half
+    uint8_t* sw = staging + (4 * cw + quad) * 4096;
+    // this warpgroup's 128 rows of A: 128 rows further down (K-major) or the third and fourth 64-wide MN blocks; 16 KB either way
+    const uint32_t a_half = (uint32_t)cw * (A_MN ? 2 * GEMM_BK * 128 : 128 * 128);
+    int stage = 0; uint32_t phase = 0;
+    auto release = [&](int s) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[s]); };
+    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+      const int split = item / tiles;
+      const int rem = item - split * tiles;
+      const int m_blk = rem / n_tiles, n_blk = rem - m_blk * n_tiles;
+      const int kb0 = split * kb_per_split;
+      const int kb1 = min(kb0 + kb_per_split, kb_total);
+      float d0[64], d1[64];                                   // accumulator rows 0-63 / 64-127 of this warpgroup's half
+#pragma unroll
+      for (int i = 0; i < 64; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+      int prev_stage = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES) + a_half;
+        const uint32_t sB = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+        wgmma_reg_fence(d0);
+        wgmma_reg_fence(d1);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / GEMM_UK; ++k) {
+          const uint64_t db = B_MN ? wgmma_desc_sw128(sB + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
+                                   : wgmma_desc_sw128(sB + k * (GEMM_UK * 2), 16, 1024);
+          const uint64_t da0 = A_MN ? wgmma_desc_sw128(sA + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
+                                    : wgmma_desc_sw128(sA + k * (GEMM_UK * 2), 16, 1024);
+          const uint64_t da1 = A_MN ? wgmma_desc_sw128(sA + GEMM_BK * 128 + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
+                                    : wgmma_desc_sw128(sA + 64 * 128 + k * (GEMM_UK * 2), 16, 1024);
+          const uint32_t acc_flag = (kb > kb0 || k > 0) ? 1u : 0u;
+          wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d0, da0, db, acc_flag);
+          wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d1, da1, db, acc_flag);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                        // the previous k-block's MMAs have retired: its smem slot is free
+        if (prev_stage >= 0) release(prev_stage);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_reg_fence(d0);
+      wgmma_reg_fence(d1);
+      if (prev_stage >= 0) release(prev_stage);
+
+      // ---- epilogue: 32-column slices, fragments -> staging tile -> one row per thread -> store_slice
+      const int wrow0 = m_blk * BM + 128 * cw + 16 * quad;
+      const int r0 = lane >> 2;
+#pragma unroll
+      for (int c = 0; c < BN / 32; ++c) {
+        const int cbase = n_blk * BN + c * 32;
+        if (cbase >= p.N) break;
+#pragma unroll
+        for (int q4 = 0; q4 < 4; ++q4) {
+          const int q = 4 * c + q4, col = 8 * q4 + 2 * (lane & 3);
+          auto put2 = [&](int rr, float x, float y) {
+            *reinterpret_cast<float2*>(sw + rr * 128 + ((((col >> 2) ^ (rr & 7))) << 4) + (col & 3) * 4) = make_float2(x, y);
+          };
+          put2(r0, d0[4 * q], d0[4 * q + 1]);
+          put2(r0 + 8, d0[4 * q + 2], d0[4 * q + 3]);
+          put2(r0 + 16, d1[4 * q], d1[4 * q + 1]);
+          put2(r0 + 24, d1[4 * q + 2], d1[4 * q + 3]);
+        }
+        __syncwarp();
+        uint32_t r[32];
+        stg_get<8>(sw, lane, r);
+        __syncwarp();
+        store_slice(p, sw, lane, r, cbase, [&](int i) { return wrow0 + (i & 15) + ((i >> 4) << 6); });
+      }
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -729,6 +924,50 @@ inline int& gemm_cluster_mode_ref() {
   return mode;
 }
 
+// split-K factor a launch really uses: clamped to [1, k-blocks], then lowered until no split is empty
+inline int gemm_effective_splits(int K, int k_splits) {
+  const int kbt = (K + GEMM_BK - 1) / GEMM_BK;
+  int s = k_splits < 1 ? 1 : k_splits > kbt ? kbt : k_splits;
+  const int per = (kbt + s - 1) / s;
+  return (kbt + per - 1) / per;
+}
+inline int gemm_kb_per_item(int K, int k_splits) { return ((K + GEMM_BK - 1) / GEMM_BK + k_splits - 1) / k_splits; }
+
+// Tile of the plain-store launches (tfx_gemm_store): mode 1 (default) the 256 x 128 cooperative tile for work items of at least
+// GEMM_WIDE_MIN_KB k-blocks when CTA pairing is off, else the 128 x 128 ping-pong tile; 2 always the wide tile; 3 never.  Set by
+// tfx_gemm_set_wide_mode (tests and tools/bench_gemm.py compare the two paths with it).
+constexpr int GEMM_WIDE_MIN_KB = 16;
+inline int& gemm_wide_mode_ref() { static int mode = 1; return mode; }
+inline bool gemm_store_wide(int K, int k_splits) {
+  const int mode = gemm_wide_mode_ref();
+  if (mode != 1) return mode == 2;
+  return gemm_cluster_mode_ref() == 1 && gemm_kb_per_item(K, gemm_effective_splits(K, k_splits)) >= GEMM_WIDE_MIN_KB;
+}
+
+template <bool A_MN, bool B_MN>
+int launch_gemm_wide_t(const GemmOperand& A, const GemmOperand& B, const GemmParams& p_in, int num_sms, cudaStream_t stream) {
+  using Cfg = GemmWideCfg;
+  GemmParams p = p_in;
+  p.K1 = p.K;
+  p.k_splits = gemm_effective_splits(p.K, p.k_splits);
+  const int items = ((p.M + Cfg::BM - 1) / Cfg::BM) * ((p.N + GEMM_BN - 1) / GEMM_BN) * p.k_splits;
+  if (items <= 0) return 0;
+  CUtensorMap tmA, tmB;
+  int rc = !A_MN ? make_tmap_bf16(&tmA, A.ptr, p.K, p.M, A.ld, Cfg::BM) : make_tmap_bf16(&tmA, A.ptr, p.M, p.K, A.ld, GEMM_BK);
+  if (rc) return rc;
+  rc = !B_MN ? make_tmap_bf16(&tmB, B.ptr, p.K, p.N, B.ld, GEMM_BN) : make_tmap_bf16(&tmB, B.ptr, p.N, p.K, B.ld, GEMM_BK);
+  if (rc) return rc;
+  auto kern = gemm_sm90_wide_kernel<A_MN, B_MN>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES) != cudaSuccess) return -2;
+    attr_set = true;
+  }
+  const int grid = items < num_sms ? items : num_sms;
+  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
+  return cudaGetLastError() == cudaSuccess ? 0 : -3;
+}
+
 template <bool A_MN, bool B_MN, int EPI>
 int launch_gemm_t(const GemmOperand& A, const GemmOperand& B, const GemmParams& p_in, int num_sms, cudaStream_t stream) {
   using Cfg = GemmCfg<EPI>;
@@ -740,18 +979,12 @@ int launch_gemm_t(const GemmOperand& A, const GemmOperand& B, const GemmParams& 
   if (!A_MN) rc = make_tmap_bf16(&tmA, A.ptr, two ? p.K1 : p.K, p.M, A.ld, GEMM_BM); else rc = make_tmap_bf16(&tmA, A.ptr, p.M, p.K, A.ld, GEMM_BK);
   if (rc) return rc;
   if (two) { rc = make_tmap_bf16(&tmA2, A.ptr2, p.K - p.K1, p.M, A.ld2, GEMM_BM); if (rc) return rc; } else tmA2 = tmA;
-  {
-    const int kbt = (p.K + GEMM_BK - 1) / GEMM_BK;
-    if (p.k_splits < 1) p.k_splits = 1;
-    if (p.k_splits > kbt) p.k_splits = kbt;
-    const int per = (kbt + p.k_splits - 1) / p.k_splits;
-    p.k_splits = (kbt + per - 1) / per;            // no empty split
-  }
+  p.k_splits = gemm_effective_splits(p.K, p.k_splits);
   const int m_tiles = (p.M + GEMM_BM - 1) / GEMM_BM, n_tiles = (p.N + GEMM_BN - 1) / GEMM_BN;
   const int items = m_tiles * n_tiles * p.k_splits;
   if (items <= 0) return 0;
   const int mode = gemm_cluster_mode_ref();
-  const int kb_item = ((p.K + GEMM_BK - 1) / GEMM_BK + p.k_splits - 1) / p.k_splits;      // k-blocks per work item
+  const int kb_item = gemm_kb_per_item(p.K, p.k_splits);      // k-blocks per work item
   const bool paired = mode == 2 || (mode == 3 && m_tiles >= 2 && kb_item >= 16 && items >= 2 * num_sms);
   // paired CTAs each fetch half of the B tile: the K-major box is 64 rows (the MN-major box is one 64-wide block either way)
   if (!B_MN) rc = make_tmap_bf16(&tmB, B.ptr, p.K, p.N, B.ld, paired ? GEMM_BN / 2 : GEMM_BN); else rc = make_tmap_bf16(&tmB, B.ptr, p.N, p.K, B.ld, GEMM_BK);

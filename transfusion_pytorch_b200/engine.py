@@ -18,6 +18,7 @@ fp32 accumulation.
 """
 from __future__ import annotations
 
+import functools
 import math
 import os
 import ctypes
@@ -104,19 +105,22 @@ def w1_row_src(inner: int) -> np.ndarray:
     return src
 
 
-def wgrad_splits(n_out, n_in, K, sms, ks):
-    """split-K factor of a wgrad GEMM over K tokens: tiles x splits should fill whole waves of the persistent grid (one CTA per SM); `ks` breaks
-    near-ties.  E.g. the [1408 x 512] FFN-out gradient has 22 tiles: 16 splits = 2.4 waves (80 % busy), 20 splits = 2.97 waves"""
-    tiles = ((n_out + 127) // 128) * ((n_in + 255) // 256 if (n_in % 256 == 0 or n_in >= 1024) else (n_in + 127) // 128)
-    best, best_eff = 1, 0.0
+@functools.lru_cache(maxsize = None)
+def wgrad_splits(n_out, n_in, K, sms):
+    """split-K factor of a wgrad GEMM (dW[n_out, n_in] over K tokens, both operands MN-major).  For each candidate the library reports the launch
+    geometry (`_lib.gemm_store_items`: the tile, and so the work items, depend on the k-blocks per item); the busiest SM then runs
+    ceil(items / sms) items of (k-blocks x tile rows / 128) units.  The fewest splits within 5 % of the shortest such path win: every split
+    adds one red.add pass over dW.  Work items keep at least 16 k-blocks.  E.g. over 131072 tokens on 132 SMs the [1664 x 512] QKVG gradient
+    has 7 x 4 = 28 tiles of 256 x 128: 9 splits are 252 items (2 waves of 228 k-blocks), 14 splits 3 waves of 147 (3 % shorter) and 4 splits
+    one 85 % wave of 512; 9 are taken."""
+    cost = {}
     for s in range(1, 65):
-        if K // s < 1024 and s > 1:
+        items, kb, tile_m, s_eff = _lib.gemm_store_items(n_out, n_in, K, 1, 1, s)
+        if s_eff != s or (s > 1 and kb < 16):
             break
-        items = tiles * s
-        eff = items / (-(-items // sms) * sms)
-        if eff > best_eff + 0.02 or (abs(eff - best_eff) <= 0.02 and s <= ks and s > best):
-            best, best_eff = s, eff
-    return best
+        cost[s] = -(-items // sms) * kb * tile_m // 128
+    best = min(cost.values())
+    return min(s for s, c in cost.items() if c <= 1.05 * best)
 
 
 class KVCache:
@@ -795,10 +799,10 @@ class Engine:
         pk, nc, S = self.packed, rb.n_cond, rb.S
         cond_row = dv['cond_row'] if nc > 0 else None
         tab_ld, zg_ld = self.W * 3 * D, self.W * D
-        ks = max(1, min(64, M // 2048))           # default split-K factor of the wgrad GEMMs (K = tokens)
+        ks = max(1, min(64, M // 2048))           # split-K cap of the latent_to_model wgrads (K = that modality's tokens)
         sms = torch.cuda.get_device_properties(self.device).multi_processor_count
         def ksplit(n_out, n_in, K = M):
-            return wgrad_splits(n_out, n_in, K, sms, ks)
+            return wgrad_splits(n_out, n_in, K, sms)
         def wgrad(dy, ld_dy, n_out, act, ld_act, n_in, gname, K = M):
             # dW[n_out, n_in] += dy^T act : both operands MN-major over the token (K) dimension, split-K atomics
             o.gemm_store(dy, ld_dy, 1, act, ld_act, 1, n_out, n_in, K, self.G(gname), n_in, None, 0, None, None, 1.0, 1, ksplit(n_out, n_in, K))
@@ -1111,10 +1115,9 @@ class RepHead:
         if g_loss is not None:
             o.scale_bf16(da, (g_loss.detach().float().reshape(1) / st['g']), da.numel())
         sms = torch.cuda.get_device_properties(eng.device).multi_processor_count
-        ks = max(1, min(64, M // 2048))
         dh = eng.buf('rh_dh', (M, Ip), BF16)
         o.gemm_store(da, D, 0, self.w2p, Ip, 1, M, Ip, D, None, 0, dh, Ip, None, None, 1.0, 0, 1)
-        o.gemm_store(da, D, 1, st['h'], Ip, 1, D, inner, M, gw2, 0, None, 0, None, self.w2_rows, 1.0, 1, wgrad_splits(D, inner, M, sms, ks))
+        o.gemm_store(da, D, 1, st['h'], Ip, 1, D, inner, M, gw2, 0, None, 0, None, self.w2_rows, 1.0, 1, wgrad_splits(D, inner, M, sms))
         o.colsum_bf16(da, D, M, D, None, gb2)
         dvg = eng.buf('rh_dvg', (M, 2 * Ip), BF16)
         rpb = o.lib.tfx_geglu_bwd_rows_per_block()
@@ -1124,7 +1127,7 @@ class RepHead:
         o.colsum_f32(part, 2 * Ip, nblk, 2 * Ip, self.b1_cols, gb1)
         du = eng.buf('rh_du', (M, D), F32)
         o.gemm_store(dvg, 2 * Ip, 0, self.w1p, D, 1, M, D, 2 * Ip, du, D, None, 0, None, None, 1.0, 0, 1)
-        o.gemm_store(dvg, 2 * Ip, 1, st['u'], D, 1, 2 * Ip, D, M, gw1, 0, None, 0, None, self.w1_rows, 1.0, 1, wgrad_splits(2 * Ip, D, M, sms, ks))
+        o.gemm_store(dvg, 2 * Ip, 1, st['u'], D, 1, 2 * Ip, D, M, gw1, 0, None, 0, None, self.w1_rows, 1.0, 1, wgrad_splits(2 * Ip, D, M, sms))
         gx = eng.buf('rh_gx', (M, D), F32)
         o.rmsnorm_bwd(du, st['x'], head[0].gamma, gx, ggamma, M, D)
         return gx
