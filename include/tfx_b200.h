@@ -20,6 +20,10 @@ extern "C" {
 
 #define TFX_B200_VERSION 200
 
+/* Deepest model the AttentionResidual kernels take: hidden-state lists hold x0 plus TFX_MAX_DEPTH layer outputs.  Transformer(...) rejects deeper
+ * models with the same number (transfusion.py MAX_DEPTH). */
+#define TFX_MAX_DEPTH 64
+
 const char* tfx_last_error(void);
 int tfx_version(void);
 int tfx_init(int device);                       /* checks the device is sm_90 */
@@ -116,7 +120,9 @@ int tfx_qk_bwd_pack(const float* dq, const float* dk, const void* q_bf16, const 
  *   G_k = sum_{i' >= k-1} [a_{i',k} dx_{i'} + c1_{i',k} w_{i'}] - (sum c2_{i',k}) h_k.
  * own = 1: layer with hiddens h_0..h_{n-1}; writes the scalars of h_0..h_{n-2} to scalars_out[token][k][3] (row stride scalar_stride floats), the parameter gradients,
  * and grad_hidden = G_{n-1} from its own term plus the n_later later layers (dx_later[j], scalars_later[j] -> element [token 0][k = n-1][0], gammas / pseudo_queries[1 + j]).
- * own = 0: assembly only (gammas[0] / pseudo_queries[0] unused): the gradient of h_0 after the first layer. */
+ * own = 0: assembly only (gammas[0] / pseudo_queries[0] unused): the gradient of h_0 after the first layer.
+ * 1 <= n_hiddens <= TFX_MAX_DEPTH + 1, 0 <= n_later <= TFX_MAX_DEPTH.  Up to 10 later layers take one launch (plus the parameter-gradient fold when own = 1);
+ * more are assembled in chunks of 10: each further launch adds its chunk's sum_j [a_j dx_j + c1_j w_j] - (sum_j c2_j) h into grad_hidden. */
 int tfx_attn_residual_bwd2(const void* const* hiddens_bf16, int n_hiddens, int own, const float* const* gammas, const float* const* pseudo_queries,
                            const float* const* dx_later, const float* const* scalars_later, int n_later, const float* dx_out, const float* x_out, const float* lse,
                            float* grad_hidden, float* scalars_out, int scalar_stride, float* dgamma, float* dpseudo_query, float* workspace, int M, int D, void* stream);
@@ -148,7 +154,8 @@ int tfx_adaln_bwd(const float* du, const float* x, const float* stats, const int
 int tfx_resid_bwd(const float* dx, const void* y_bf16, const int* cond_row, const float* zgate, long long zgate_ld, const float* layerscale,
                   void* dy_bf16, float* dzgate, long long dzgate_ld, float* dlayerscale, float* dbias, int M, int D, void* stream);
 /* AttentionResidual (T.py:803-829): softmax mix over all hiddens so far, single pass; lse_out [M] (optional) = log-sum-exp of the
- * depth softmax, consumed by the backward together with the forward output x_out so that every hidden is read exactly once */
+ * depth softmax, consumed by the backward together with the forward output x_out so that every hidden is read exactly once.
+ * 1 <= n_hiddens <= TFX_MAX_DEPTH + 1 (forward and accumulating backward). */
 int tfx_attn_residual_fwd(const float* const* hiddens, int n_hiddens, const float* gamma, const float* pseudo_query,
                           float* x_out, void* x_out_bf16, float* lse_out, int M, int D, void* stream);
 long long tfx_attn_residual_bwd_workspace_floats(int M, int D);   /* fp32 scratch for the per-block parameter-gradient partial sums */

@@ -1,0 +1,331 @@
+"""GPU (H100): models deeper than ten layers, up to the depth limit of 64.
+
+  * the AttentionResidual kernels against float64: forward with 33 and 65 hiddens, accumulating backward with 65, and the deferred backward chain at
+    depth 11, 23 and 64, which crosses every chunk boundary of its assembly (10 -> 11 and 20 -> 21 later layers) and the x0 assembly;
+  * whole models against the reference fixtures of oracle/make_golden_deep.py, at the tolerances of tests/test_parity_gpu.py;
+  * one train step at size against the fp32 checker (oracle/torch_reference.py), and the deferred against the accumulating backward;
+  * CUDA-graph replay and Self-Flow at depth 12;
+  * depth <= 10 keeps one deferred-backward launch per call."""
+import ctypes
+
+import pytest
+import torch
+
+from helpers import load_golden, golden_noise, grad_fingerprint, unpack_rows
+from oracle.make_golden_deep import INTERLEAVED, deep_batch
+from oracle.torch_reference import OracleEngine
+from test_dropout_gpu import _launches
+from test_parity_gpu import LOSS_REL, build, check_grads, rel_max, HID_REL, GRAD_REL
+from test_selfflow_cpu import grads_close
+from transfusion_pytorch_b200 import Transfusion, SelfMaskedRepTraining, _lib, synth
+
+pytestmark = pytest.mark.gpu
+BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
+
+
+@pytest.fixture(scope = 'module')
+def ops():
+    return _lib.Ops()
+
+
+class Ptrs:
+    """ctypes pointer arrays kept alive for the duration of a test"""
+
+    def __init__(self):
+        self.keep = []
+
+    def __call__(self, ts):
+        a = (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+        self.keep.append(a)
+        return ctypes.cast(a, ctypes.c_void_p)
+
+
+def ares_ref(hs, gam, pq):
+    """float64 AttentionResidual (T.py:803-829): x = sum_l softmax_l(<normalize(h_l) sqrt(D) (gam + 1), pq> / sqrt(D)) h_l, and the log-sum-exp"""
+    vals = torch.stack(hs)
+    D = vals.shape[-1]
+    keys = torch.nn.functional.normalize(vals, dim = -1) * D ** 0.5 * (gam + 1)
+    sim = torch.einsum('lnd,d->nl', keys, pq) * D ** -0.5
+    return torch.einsum('nl,lnd->nd', sim.softmax(-1), vals), sim.logsumexp(-1)
+
+
+def rand_inputs(n_hid, M, D, seed):
+    g = torch.Generator(device = 'cuda').manual_seed(seed)
+    hid = [torch.randn(M, D, device = 'cuda', generator = g).to(BF16).float() for _ in range(n_hid)]
+    return hid, torch.randn(D, device = 'cuda', generator = g) * 0.3, torch.randn(D, device = 'cuda', generator = g) * 0.5
+
+
+@pytest.mark.parametrize('hb', [False, True], ids = ['fp32', 'bf16'])
+@pytest.mark.parametrize('n_hid', [33, 65])
+@pytest.mark.parametrize('D', [128, 512, 1024])
+def test_attn_residual_fwd_deep_vs_float64(ops, hb, n_hid, D):
+    M = 1500
+    hid, gam, pq = rand_inputs(n_hid, M, D, seed = n_hid + D)
+    src = [h.to(BF16) for h in hid] if hb else hid
+    P = Ptrs()
+    xo = torch.full((M, D), 7., device = 'cuda'); xb = torch.full((M, D), 7., device = 'cuda', dtype = BF16); lse = torch.full((M,), 7., device = 'cuda')
+    (ops.attn_residual_fwd_h16 if hb else ops.attn_residual_fwd)(P(src), n_hid, gam, pq, xo, xb, lse, M, D)
+    torch.cuda.synchronize()
+    want, want_lse = ares_ref([h.double() for h in hid], gam.double(), pq.double())
+    assert ((xo.double() - want).abs().max() / want.abs().max()).item() < 1e-5
+    assert torch.equal(xb, xo.to(BF16))
+    assert (lse.double() - want_lse).abs().max().item() < 1e-5
+
+
+@pytest.mark.parametrize('D', [128, 512, 1024])
+def test_attn_residual_accumulating_bwd_65_hiddens_vs_float64(ops, D):
+    n_hid, M = 65, 700
+    hid, gam, pq = rand_inputs(n_hid, M, D, seed = 5 + D)
+    R = torch.randn(M, D, device = 'cuda', generator = torch.Generator(device = 'cuda').manual_seed(9))
+    h64 = [h.double().requires_grad_(True) for h in hid]
+    g64, p64 = gam.double().requires_grad_(True), pq.double().requires_grad_(True)
+    x, _ = ares_ref(h64, g64, p64)
+    (x * R.double()).sum().backward()
+    P = Ptrs()
+    xo = torch.zeros(M, D, device = 'cuda'); lse = torch.zeros(M, device = 'cuda')
+    hb = [h.to(BF16) for h in hid]
+    ops.attn_residual_fwd_h16(P(hb), n_hid, gam, pq, xo, None, lse, M, D)
+    dH = [torch.full((M, D), 7., device = 'cuda') for _ in range(n_hid)]
+    dgam, dpq = torch.zeros(D, device = 'cuda'), torch.zeros(D, device = 'cuda')
+    ws = torch.zeros(int(ops.lib.tfx_attn_residual_bwd_workspace_floats(M, D)), device = 'cuda')
+    ops.attn_residual_bwd_h16(P(hb), P(dH), n_hid, gam, pq, R, xo, lse, dgam, dpq, ws, M, D, 1)
+    torch.cuda.synchronize()
+    for k in range(n_hid):
+        err = (dH[k].double() - h64[k].grad).abs().max().item() / h64[k].grad.abs().max().item()
+        assert err < 2e-3, (k, err)
+    assert torch.allclose(dgam.double(), g64.grad, atol = 5e-3, rtol = 1e-2) and torch.allclose(dpq.double(), p64.grad, atol = 5e-3, rtol = 1e-2)
+
+
+@pytest.mark.parametrize('depth', [11, 23, 64])
+@pytest.mark.parametrize('D', [128, 512, 1024])
+def test_attn_residual_deferred_chain_deep_vs_float64(ops, depth, D):
+    """tfx_attn_residual_bwd2 over a stack of `depth` AttentionResiduals (layer i mixes h_0 .. h_{i+1}), loss = sum_i <x_i, R_i>, as in
+    tests/test_ops_gpu.py::test_attn_residual_deferred_backward_chain_vs_autograd: every hidden's assembled gradient must equal float64 autograd's
+    sum over the layers.  Layer i has depth - 1 - i later layers and the x0 assembly has depth, so the chunked launches are all exercised."""
+    M = 600 if D * depth <= 23 * 512 else (256 if depth < 64 else 128)         # float64 autograd keeps every layer's stacked hiddens
+    g = torch.Generator(device = 'cuda').manual_seed(depth * 7 + D)
+    hid = [torch.randn(M, D, device = 'cuda', generator = g).to(BF16).double().requires_grad_(True) for _ in range(depth + 1)]
+    gams = [(torch.randn(D, device = 'cuda', generator = g) * 0.3).double().requires_grad_(True) for _ in range(depth)]
+    pqs = [(torch.randn(D, device = 'cuda', generator = g) * 0.5).double().requires_grad_(True) for _ in range(depth)]
+    R = [torch.randn(M, D, device = 'cuda', generator = g) for _ in range(depth)]
+    loss = 0.
+    for i in range(depth):
+        loss = loss + (ares_ref(hid[:i + 2], gams[i], pqs[i])[0] * R[i].double()).sum()
+    loss.backward()
+    del loss
+    P = Ptrs()
+    hb = [h.detach().to(BF16) for h in hid]
+    gd, pd = [t.detach().float() for t in gams], [t.detach().float() for t in pqs]
+    xo = [torch.zeros(M, D, device = 'cuda') for _ in range(depth)]; lse = [torch.zeros(M, device = 'cuda') for _ in range(depth)]
+    for i in range(depth):
+        ops.attn_residual_fwd_h16(P(hb[:i + 2]), i + 2, gd[i], pd[i], xo[i], None, lse[i], M, D)
+    stride = (depth + 2) * 3
+    sc = torch.zeros(depth, M, depth + 2, 3, device = 'cuda')
+    G = [torch.full((M, D), 7., device = 'cuda') for _ in range(depth + 1)]
+    dgam = [torch.zeros(D, device = 'cuda') for _ in range(depth)]; dpq = [torch.zeros(D, device = 'cuda') for _ in range(depth)]
+    ws = torch.zeros(int(ops.lib.tfx_attn_residual_bwd_workspace_floats(M, D)), device = 'cuda')
+    for i in reversed(range(depth)):
+        later = list(range(i + 1, depth))
+        ops.attn_residual_bwd2(P(hb[:i + 2]), i + 2, 1, P([gd[j] for j in [i] + later]), P([pd[j] for j in [i] + later]), P([R[j] for j in later] or [R[i]]),
+                               P([sc[j][0, i + 1] for j in later] or [R[i]]), len(later), R[i], xo[i], lse[i], G[i + 1], sc[i], stride, dgam[i], dpq[i], ws, M, D)
+    ops.attn_residual_bwd2(P(hb[:1]), 1, 0, P([gd[0]] + gd), P([pd[0]] + pd), P(R), P([sc[j][0, 0] for j in range(depth)]), depth, None, None, None, G[0], None,
+                           stride, None, None, None, M, D)
+    torch.cuda.synchronize()
+    for k in range(depth + 1):
+        err = (G[k].double() - hid[k].grad).abs().max().item() / hid[k].grad.abs().max().item()
+        assert err < 2e-3, (k, err)
+    for i in range(depth):
+        assert torch.allclose(dgam[i].double(), gams[i].grad, atol = 5e-3, rtol = 1e-2) and torch.allclose(dpq[i].double(), pqs[i].grad, atol = 5e-3, rtol = 1e-2), i
+
+
+# ---------------------------------------------------------------------------------------------------- whole model against the reference
+@pytest.mark.parametrize('name,depth,seed,total_len', INTERLEAVED, ids = [c[0] for c in INTERLEAVED])
+def test_deep_train_step_matches_reference(name, depth, seed, total_len):
+    fx = load_golden(name)
+    model = build(fx)
+    assert model.transformer.depth == depth
+    batch = deep_batch(seed, total_len)
+    loss, bd = model(batch, times = fx['times'], return_breakdown = True, noise = golden_noise(fx, batch, model.dim_latents))
+    rb = model._last_batch
+    assert rb.modality_positions == fx['modality_positions'] and rb.total_tokens == fx['total_tokens']
+    assert abs(loss.item() - fx['loss'].item()) / fx['loss'].item() < LOSS_REL
+    assert abs(bd.text.item() - fx['text_loss'].item()) / fx['text_loss'].item() < LOSS_REL
+    for a, b in zip(bd.flow, fx['flow_losses']):
+        assert abs(a.item() - b.item()) / b.item() < LOSS_REL
+    st = model.engine.state
+    rows = fx['hidden_rows']                 # the fixture keeps every hidden state at these positions
+    for l, h in enumerate(fx['hiddens']):
+        ours = unpack_rows(st['hid'][l], rb)
+        for b in range(rb.B):
+            keep = rows < int(rb.seq_lens[b])
+            assert rel_max(ours[b, rows[keep]], h[b, keep]) < HID_REL, f'hidden {l} sample {b}'
+    emb = unpack_rows(st['out'], rb)
+    for b in range(rb.B):
+        n = int(rb.seq_lens[b])
+        assert rel_max(emb[b, :n], fx['embed'][b, :n]) < HID_REL
+    loss.backward()
+    check_grads(model, fx)
+
+
+def test_deep_text_only_loss_grads_and_greedy_tokens():
+    fx = load_golden('text_deep12')
+    model = build(fx)
+    text = synth.text_batch(4, 129, seed = 12)
+    loss = model(text)
+    assert abs(loss.item() - fx['loss'].item()) / fx['loss'].item() < LOSS_REL
+    loss.backward()
+    check_grads(model, fx)
+    ref = fx['generated']
+    seq = torch.cat((text[:, :fx['prompt_len']], ref), dim = -1)
+    with torch.no_grad():
+        lg = model.forward_text(seq[:, :-1], return_loss = False).float()
+    pred = lg[:, fx['prompt_len'] - 1:].argmax(dim = -1).cpu()
+    decided = fx['margins'] >= 0.1
+    assert decided.float().mean().item() > 0.5
+    assert torch.equal(pred[decided], ref[decided])
+    # free-running greedy decode through the kv cache: identical up to the first position whose reference margin is below 0.1
+    gen = model.generate_text_only(text[:, :fx['prompt_len']], fx['gen_len'], temperature = 0.).cpu()
+    for b in range(gen.shape[0]):
+        for j in range(gen.shape[1]):
+            if gen[b, j] != ref[b, j]:
+                assert fx['margins'][b, j] < 0.1, (b, j)
+                break
+
+
+# ---------------------------------------------------------------------------------------------------- at size against the checker
+def _config(D, depth):
+    return dict(num_text_tokens = 256, dim_latent = (64, 32), modality_default_shape = ((4,), (2,)), prob_uncond = 0.,
+                transformer = dict(dim = D, depth = depth, heads = D // 64))
+
+
+def _step(model, batch, times, noise):
+    loss = model(batch, times = times, noise = noise)
+    loss.backward()
+    return loss.item(), grad_fingerprint((n, p.grad) for n, p in model.named_parameters() if p.grad is not None)
+
+
+def _close(got, want, what):
+    (lg, fg), (lw, fw) = got, want
+    assert abs(lg - lw) / abs(lw) < LOSS_REL, (what, lg, lw)
+    grads_close(fg, fw, GRAD_REL)
+
+
+@pytest.mark.parametrize('D,depth,total_len', [(768, 12, 1024), (1024, 24, 512), (128, 64, 1024)])
+def test_deep_train_step_at_size_matches_checker(D, depth, total_len):
+    ctor = _config(D, depth)
+    batch = synth.config4_batch(2, seed = 41, total_len = total_len, dims = (64, 32))
+    nm = max(sum(isinstance(p, tuple) for p in s) for s in batch)
+    times = torch.rand(2, nm, generator = torch.Generator().manual_seed(3))
+    rows = [sum(p[1].shape[0] for s in batch for p in s if isinstance(p, tuple) and p[0] == t) for t in range(2)]
+    noise = [torch.randn(max(r, 1), dl, generator = torch.Generator().manual_seed(10 + t)) for t, (r, dl) in enumerate(zip(rows, (64, 32)))]
+    res = {}
+    for mode in (['cpu', 'deferred', 'accumulating'] if depth == 24 else ['cpu', 'deferred']):
+        torch.manual_seed(0)
+        model = Transfusion(**ctor)
+        synth.fill_parameters_(model, seed = 4)
+        model = model.to('cpu' if mode == 'cpu' else 'cuda').eval()
+        if mode == 'cpu':
+            model._engine = OracleEngine(model)
+        else:
+            model.engine.ares_deferred = mode == 'deferred'
+        res[mode] = _step(model, batch, times, noise)
+        del model
+        torch.cuda.empty_cache()
+    _close(res['deferred'], res['cpu'], 'deferred')
+    if 'accumulating' in res:
+        _close(res['accumulating'], res['cpu'], 'accumulating')
+        _close(res['deferred'], res['accumulating'], 'deferred vs accumulating')
+
+
+# ---------------------------------------------------------------------------------------------------- paths
+DEEP12 = dict(num_text_tokens = 64, dim_latent = 32, modality_default_shape = (4,), prob_uncond = 0., transformer = dict(dim = 128, depth = 12, heads = 2))
+
+
+def _model(ctor, seed):
+    torch.manual_seed(0)
+    model = Transfusion(**ctor)
+    synth.fill_parameters_(model, seed = seed)
+    return model.cuda()
+
+
+def test_deep_graph_replay_follows_eager():
+    from transfusion_pytorch_b200.data_parallel import DataParallelTrainer
+    from transfusion_pytorch_b200.modality_processing import pack_batch
+    batch = synth.dropout_batch()
+    times = torch.rand(3, 2, generator = torch.Generator().manual_seed(5))
+    results = []
+    for use_graph in (False, True):
+        model = _model(DEEP12, 7).train()
+        trn = DataParallelTrainer(model, lr = 1e-3, cuda_graph = use_graph)
+        eng = model.engine
+        eng.ensure_attached()
+        samples = [[torch.tensor([model.sos_id]), *s, torch.tensor([model.eos_id])] for s in batch]
+        rb = pack_batch(samples, times, model, return_loss = True, return_embed = False)
+        lat = model._latents_to_device(rb)
+        eng.upload(rb)
+        losses = []
+        for step in range(6):
+            noise = [torch.randn(52, 32, generator = torch.Generator().manual_seed(500 + step)).cuda()]
+            losses.append(trn.step_packed(rb, lat, noise = noise).item())
+        results.append((losses, eng.flat.clone()))
+        if use_graph:
+            assert sum(g.graph is not None for g in trn._graphs.values()) == 1, 'the step was never captured'
+    (l0, p0), (l1, p1) = results
+    assert all(abs(a - b) / abs(a) < 2e-3 for a, b in zip(l0, l1)), (l0, l1)
+    assert (p1 - p0).abs().max().item() < 2e-3 * p0.abs().max().item() + 2e-4
+
+
+def test_deep_self_flow_matches_checker():
+    from oracle.selfflow_reference import selfflow_loss
+    batch = synth.small_batch(3, seed = 1, dim_latent = 32, text_vocab = 64)
+    nm = max(sum(torch.is_tensor(p) and p.is_floating_point() for p in s) for s in batch)
+    times = torch.rand(3, nm, generator = torch.Generator().manual_seed(5))
+    rows = sum(p.shape[0] for s in batch for p in s if torch.is_tensor(p) and p.is_floating_point())
+    noise = [torch.randn(rows, 32, generator = torch.Generator().manual_seed(3))]
+    tnoise = [torch.randn(rows, 32, generator = torch.Generator().manual_seed(8))]
+    res = {}
+    for dev in ('cuda', 'cpu'):
+        torch.manual_seed(0)
+        model = Transfusion(**DEEP12)
+        synth.fill_parameters_(model, seed = 4)
+        wrapper = SelfMaskedRepTraining(model.to(dev), use_asymmetric_dropout = False, student_layer = -3).to(dev)
+        synth.fill_parameters_(wrapper.student_predict_head, seed = 6)
+        if dev == 'cuda':
+            total, (student, ssl) = wrapper(batch, times = times, noise = noise, teacher_noise = tnoise)
+        else:
+            total, student, ssl = selfflow_loss(wrapper, batch, times, noise, tnoise)
+        total.backward()
+        named = [(n, p.grad) for n, p in wrapper.student.named_parameters() if p.grad is not None]
+        named += [(f'student_predict_head.{n}', p.grad) for n, p in wrapper.student_predict_head.named_parameters()]
+        res[dev] = (total.item(), student.item(), ssl.item(), grad_fingerprint(named))
+    for k in range(3):
+        assert abs(res['cuda'][k] - res['cpu'][k]) / abs(res['cpu'][k]) < LOSS_REL, (k, res['cuda'][k], res['cpu'][k])
+    grads_close(res['cuda'][3], res['cpu'][3], GRAD_REL)
+
+
+# ---------------------------------------------------------------------------------------------------- launches
+def _bwd2_kernels(model, batch, times, noise):
+    """(n_later of every attn_residual_bwd2 call, number of attn_res_bwd2_k kernels) of one train step"""
+    _, calls = _launches(model, batch, times, noise)
+    n_later = [args[7] for args in calls['attn_residual_bwd2']]
+    with torch.profiler.profile(activities = [torch.profiler.ProfilerActivity.CUDA]) as prof:
+        loss = model(batch, times = times, noise = noise)
+        loss.backward()
+        torch.cuda.synchronize()
+    kernels = sum(e.count for e in prof.key_averages() if 'attn_res_bwd2_k' in e.key)
+    return n_later, kernels
+
+
+@pytest.mark.parametrize('depth', [8, 12])
+def test_deferred_backward_launches(depth):
+    """depth <= 10: one kernel per attn_residual_bwd2 call, as before chunking; deeper: one per started chunk of 10 later layers"""
+    ctor = dict(DEEP12, transformer = dict(DEEP12['transformer'], depth = depth))
+    batch = synth.dropout_batch()
+    times = torch.rand(3, 2, generator = torch.Generator().manual_seed(5))
+    noise = [torch.randn(52, 32, generator = torch.Generator().manual_seed(1))]
+    n_later, kernels = _bwd2_kernels(_model(ctor, 3).eval(), batch, times, noise)
+    assert sorted(n_later) == sorted(list(range(depth)) + [depth])
+    if depth <= 10:
+        assert max(n_later) <= 10 and len(n_later) == depth + 1 and kernels == depth + 1
+    else:
+        assert kernels == sum(max(1, -(-n // 10)) for n in n_later)

@@ -10,7 +10,8 @@
 
 namespace tfx {
 
-struct PtrList { float* p[32]; };
+constexpr int MAX_HIDDENS = TFX_MAX_DEPTH + 1;    // x0 and every layer output: 65 pointers, 520 B of kernel parameters
+struct PtrList { float* p[MAX_HIDDENS]; };
 
 // ------------------------------------------------------------------------------------ adaLN forward
 // u = isM ? LN(x)*(gamma_c+1)+beta_c : LN(x)*(g+1)      (T.py:747-755; text-only 677-679)
@@ -399,12 +400,15 @@ __global__ void __launch_bounds__(ROW_THREADS, 2) attn_res_bwd_k(PtrList hid, Pt
 //     G_k = sum_{i' >= k-1} [ a_{i',k} dx_{i'} + c1_{i',k} w_{i'} ] - (sum_{i'} c2_{i',k}) h_k
 // Layer i (own = 1): scalar pass over h_0 .. h_{i+1} (parameter gradients, scalars out), then G_{i+1} from its own term and the stored scalars / incoming
 // gradients of the later layers.  own = 0: only the assembly (G_0, after the first layer).  Bytes per token over 8 layers: 167 KB instead of 234 KB.
+// One launch assembles at most BWD2_CHUNK later layers (their w rows in shared memory, one lane each for their scalars).  The sum is linear in the
+// later layers, so deeper models add the rest chunk by chunk: ACC launches (own = 0) add their chunk's terms, c2 part included, into G.
+constexpr int BWD2_CHUNK = 10;
 struct ResBwd2Args {
-  const __nv_bfloat16* hid[12];     // bf16 hiddens h_0 .. h_{L1-1}
-  const float* dx_later[10];        // incoming gradients of the later AttentionResiduals (layers i+1 ..)
-  const float* sc_later[10];        // their scalars for THIS hidden: points at element [token 0][k = L1-1][0]; row stride = sc_stride floats
-  const float* gam[11];             // norm_keys.gamma: own layer first (unused when own = 0), then the later layers
-  const float* pq[11];
+  const __nv_bfloat16* hid[MAX_HIDDENS];   // bf16 hiddens h_0 .. h_{L1-1}
+  const float* dx_later[BWD2_CHUNK];        // incoming gradients of the later AttentionResiduals (layers i+1 ..)
+  const float* sc_later[BWD2_CHUNK];        // their scalars for THIS hidden: points at element [token 0][k = L1-1][0]; row stride = sc_stride floats
+  const float* gam[BWD2_CHUNK + 1];         // norm_keys.gamma: own layer first (unused when own = 0), then the later layers
+  const float* pq[BWD2_CHUNK + 1];
   int L1, n_later, own;
 };
 
@@ -414,7 +418,7 @@ struct ResBwd2Args {
 // flight (a register prefetch keeps only one).
 template <int NCH> struct ResBwd2Cfg { static constexpr int RING = NCH <= 4 ? 5 : 3; };
 
-template <int NCH>
+template <int NCH, bool ACC>
 __global__ void __launch_bounds__(ROW_THREADS, 2) attn_res_bwd2_k(ResBwd2Args A, const float* __restrict__ dxo, const float* __restrict__ xo, const float* __restrict__ lse,
                                                                  float* __restrict__ G, float* __restrict__ sc_out, int sc_stride, float* __restrict__ partials, int M, int tpw) {
   constexpr int D = NCH * 128;
@@ -558,6 +562,11 @@ __global__ void __launch_bounds__(ROW_THREADS, 2) attn_res_bwd2_k(ResBwd2Args A,
     }
 #pragma unroll
     for (int i = 0; i < NCH * 4; ++i) g[i] -= c2sum * h[i];
+    if (ACC) {                                      // a further chunk of later layers: add to what the earlier launches stored
+      load_row_f32<NCH>(G + (long long)row * D, lane, h);
+#pragma unroll
+      for (int i = 0; i < NCH * 4; ++i) g[i] += h[i];
+    }
     store_row_f32<NCH>(G + (long long)row * D, lane, g);
   }
   asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -951,7 +960,7 @@ int tfx_resid_bwd(const float* dx, const void* y_bf16, const int* cond_row, cons
 static int attn_residual_fwd_impl(const void* const* hiddens, bool hb, int n_hiddens, const float* gamma, const float* pseudo_query,
                                   float* x_out, void* x_out_bf16, float* lse_out, int M, int D, void* stream) {
   if (M <= 0) return 0;
-  TFX_REQUIRE(n_hiddens >= 1 && n_hiddens <= 32, "attn_residual: n_hiddens %d out of range [1,32]", n_hiddens);
+  TFX_REQUIRE(n_hiddens >= 1 && n_hiddens <= MAX_HIDDENS, "attn_residual: n_hiddens %d out of range [1,%d]", n_hiddens, MAX_HIDDENS);
   PtrList pl;
   for (int i = 0; i < n_hiddens; ++i) pl.p[i] = reinterpret_cast<float*>(const_cast<void*>(hiddens[i]));
   // persistent grid: exactly the resident blocks (registers / ring shared memory decide), rows strided over all warps
@@ -989,7 +998,7 @@ static int attn_residual_bwd_impl(const void* const* hiddens, bool hb, float* co
                                   const float* dx_out, const float* x_out, const float* lse, float* dgamma, float* dpseudo_query, float* workspace, int M, int D, int init,
                                   void* stream) {
   if (M <= 0) return 0;
-  TFX_REQUIRE(n_hiddens >= 1 && n_hiddens <= 32, "attn_residual: n_hiddens %d out of range [1,32]", n_hiddens);
+  TFX_REQUIRE(n_hiddens >= 1 && n_hiddens <= MAX_HIDDENS, "attn_residual: n_hiddens %d out of range [1,%d]", n_hiddens, MAX_HIDDENS);
   TFX_REQUIRE(workspace != nullptr, "attn_residual_bwd: workspace of tfx_attn_residual_bwd_workspace_floats(M, D) floats is required");
   PtrList pl, dl;
   for (int i = 0; i < n_hiddens; ++i) { pl.p[i] = reinterpret_cast<float*>(const_cast<void*>(hiddens[i])); dl.p[i] = dhiddens[i]; }
@@ -1017,25 +1026,37 @@ int tfx_attn_residual_bwd2(const void* const* hiddens_bf16, int n_hiddens, int o
                            const float* const* dx_later, const float* const* scalars_later, int n_later, const float* dx_out, const float* x_out, const float* lse,
                            float* grad_hidden, float* scalars_out, int scalar_stride, float* dgamma, float* dpseudo_query, float* workspace, int M, int D, void* stream) {
   if (M <= 0) return 0;
-  TFX_REQUIRE(n_hiddens >= 1 && n_hiddens <= 12 && n_later >= 0 && n_later <= 10, "attn_residual_bwd2: %d hiddens / %d later layers out of range", n_hiddens, n_later);
+  TFX_REQUIRE(n_hiddens >= 1 && n_hiddens <= MAX_HIDDENS && n_later >= 0 && n_later <= TFX_MAX_DEPTH, "attn_residual_bwd2: %d hiddens / %d later layers out of range [1,%d] / [0,%d]",
+              n_hiddens, n_later, MAX_HIDDENS, TFX_MAX_DEPTH);
   TFX_REQUIRE(!own || workspace != nullptr, "attn_residual_bwd2: workspace of tfx_attn_residual_bwd_workspace_floats(M, D) floats is required");
-  ResBwd2Args A;
-  memset(&A, 0, sizeof(A));
-  A.L1 = n_hiddens; A.n_later = n_later; A.own = own ? 1 : 0;
-  for (int i = 0; i < n_hiddens; ++i) A.hid[i] = reinterpret_cast<const __nv_bfloat16*>(hiddens_bf16[i]);
-  for (int j = 0; j <= n_later; ++j) { A.gam[j] = gammas[j]; A.pq[j] = pseudo_queries[j]; }
-  for (int j = 0; j < n_later; ++j) { A.dx_later[j] = dx_later[j]; A.sc_later[j] = scalars_later[j]; }
   const int tpw = ATTN_RES_BWD2_TPW;
   const int blocks = chunk_grid(M, tpw);
-  const int slots = (1 + n_later) > WARPS_PER_BLOCK ? (1 + n_later) : WARPS_PER_BLOCK;
-  TFX_DISPATCH_NCH(D, {
-    const size_t smem = (size_t)(slots + WARPS_PER_BLOCK * ResBwd2Cfg<NCH>::RING) * D * sizeof(float);
-    auto kern = attn_res_bwd2_k<NCH>;
-    static bool attr_set = false;                 // (one flag per NCH instantiation; the size below is the maximum any call can ask for)
-    if (!attr_set) { cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((11 + WARPS_PER_BLOCK * ResBwd2Cfg<NCH>::RING) * D * sizeof(float))); attr_set = true; }
-    kern<<<blocks, ROW_THREADS, smem, ST(stream)>>>(A, dx_out, x_out, lse, grad_hidden, scalars_out, scalar_stride, workspace, M, tpw);
-  });
-  if (int rc = check_launch("attn_residual_bwd2")) return rc;
+  // launch c covers later layers [j0, j0 + n): c = 0 is the full kernel (own term, scalars, parameter gradients when own = 1) and stores G; every
+  // further chunk is an own = 0 assembly whose gammas / pseudo-queries start one slot early (slot 0 unused), so the kernel sees them as 1 .. n
+  for (int j0 = 0; j0 == 0 || j0 < n_later; j0 += BWD2_CHUNK) {
+    const int n = n_later - j0 < BWD2_CHUNK ? n_later - j0 : BWD2_CHUNK;
+    const bool acc = j0 > 0;
+    ResBwd2Args A;
+    memset(&A, 0, sizeof(A));
+    A.L1 = n_hiddens; A.n_later = n; A.own = (own && !acc) ? 1 : 0;
+    for (int i = 0; i < n_hiddens; ++i) A.hid[i] = reinterpret_cast<const __nv_bfloat16*>(hiddens_bf16[i]);
+    for (int j = 0; j <= n; ++j) { A.gam[j] = gammas[j0 + j]; A.pq[j] = pseudo_queries[j0 + j]; }
+    for (int j = 0; j < n; ++j) { A.dx_later[j] = dx_later[j0 + j]; A.sc_later[j] = scalars_later[j0 + j]; }
+    const int slots = (1 + n) > WARPS_PER_BLOCK ? (1 + n) : WARPS_PER_BLOCK;
+    TFX_DISPATCH_NCH(D, {
+      const size_t smem = (size_t)(slots + WARPS_PER_BLOCK * ResBwd2Cfg<NCH>::RING) * D * sizeof(float);
+      const int smem_max = (int)((BWD2_CHUNK + 1 + WARPS_PER_BLOCK * ResBwd2Cfg<NCH>::RING) * D * sizeof(float));
+      static bool attr_set = false;               // (one flag per NCH instantiation; the size above is the maximum any call can ask for)
+      if (!attr_set) {
+        cudaFuncSetAttribute(attn_res_bwd2_k<NCH, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
+        cudaFuncSetAttribute(attn_res_bwd2_k<NCH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
+        attr_set = true;
+      }
+      if (acc) attn_res_bwd2_k<NCH, true><<<blocks, ROW_THREADS, smem, ST(stream)>>>(A, dx_out, x_out, lse, grad_hidden, scalars_out, scalar_stride, workspace, M, tpw);
+      else attn_res_bwd2_k<NCH, false><<<blocks, ROW_THREADS, smem, ST(stream)>>>(A, dx_out, x_out, lse, grad_hidden, scalars_out, scalar_stride, workspace, M, tpw);
+    });
+    if (int rc = check_launch("attn_residual_bwd2")) return rc;
+  }
   if (own) {
     const int rpb = 16;
     attn_res_bwd_finish_k<<<dim3((D + 127) / 128, (blocks + rpb - 1) / rpb), 128, 0, ST(stream)>>>(workspace, blocks, D, gammas[0], pseudo_queries[0], dgamma, dpseudo_query, rpb);

@@ -27,6 +27,9 @@ from ._pinned import POOL
 from .modality_processing import (
     ModalitySample, RaggedBatch, pack_batch, pack_text_only, pack_incremental, get_processing_strategy, DEFAULT_PROCESSING_STRATEGY, is_int_tensor)
 
+# Deepest model the AttentionResidual kernels take (TFX_MAX_DEPTH in include/tfx_b200.h): their hidden-state lists hold x0 and 64 layer outputs
+MAX_DEPTH = 64
+
 
 class TextKVCache:
     """Handle returned as the first element of the reference's `(kv_cache, tokens_seen)` tuple (T.py:2613, 2636): B cache slabs that grow in place."""
@@ -204,6 +207,7 @@ class Transformer(Module):
         super().__init__()
         unsupported = []
         if dim_head != 64: unsupported.append('dim_head != 64')
+        if depth > MAX_DEPTH: unsupported.append(f'depth {depth} > {MAX_DEPTH}')
         ff_dropout = float(ff_kwargs.get('dropout', 0.))
         for name, p in (('dropout', dropout), ("ff_kwargs['dropout']", ff_dropout)):
             if not 0. <= p <= 1.:
