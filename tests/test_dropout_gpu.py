@@ -28,7 +28,7 @@ def ffn_keep(key, p, layer, M, cols):
 
 
 def geglu_inputs(M, D = 512, inner = 1365, seed = 13):
-    """packed W1 / bias as the engine lays them out (tile t = [64 value | 64 gate] columns), as in tests/test_gemm_pingpong_gpu.py"""
+    """packed W1 / bias as the engine lays them out (tile t = [64 value | 64 gate] columns), as in tests/test_block_epilogues_gpu.py"""
     g = torch.Generator(device = 'cuda').manual_seed(seed)
     Ip = (inner + 63) // 64 * 64
     W1 = torch.randn(2 * inner, D, device = 'cuda', generator = g) / D ** 0.5

@@ -228,135 +228,6 @@ def test_ce_and_mse_heads_vs_torch(ops):
     assert torch.allclose(dl[:, :V].float(), lg.grad, atol = 2e-3, rtol = 1e-2) and (dl[:, V:] == 0).all()
 
 
-# ================================================================================================ fused GEMM epilogues vs fp32 torch
-def _rope_tables(ops, n_pos):
-    freqs = 1. / (10000 ** (torch.arange(0, 64, 2, device = 'cuda').float() / 64))
-    t = torch.empty(n_pos, 32, 2, device = 'cuda'); tt = torch.empty(32, n_pos, 2, device = 'cuda')
-    ops.rope_table(freqs, t, tt, n_pos, 32)
-    return freqs, t, tt
-
-
-def _rope_ref(x, pos, freqs):                       # interleaved pairs (x0, x1) -> (x0 c - x1 s, x1 c + x0 s)
-    ang = (pos[:, None].float() * freqs).repeat_interleave(2, dim = -1)            # [M, 64]
-    x2 = x.reshape(*x.shape[:-1], 32, 2)
-    rot = torch.stack((-x2[..., 1], x2[..., 0]), dim = -1).flatten(-2)
-    return x * ang.cos()[:, None] + rot * ang.sin()[:, None]
-
-
-@pytest.mark.parametrize('M,H,D', [(700, 8, 512), (300, 2, 128), (257, 4, 256)])
-def test_gemm_qkvg_epilogue_vs_torch(ops, cluster_mode, M, H, D):
-    """to_qk | to_v | to_gates GEMM + per-head qk-RMSNorm + interleaved RoPE (T.py:946-965, 1027), incl. the kv-cache row scatter"""
-    g = torch.Generator(device = 'cuda').manual_seed(4)
-    HI, NQ = H * 64, 3 * H * 64 + 128
-    u = torch.randn(M, D, device = 'cuda', generator = g).to(BF16)
-    W = torch.zeros(NQ, D, device = 'cuda', dtype = BF16)
-    W[:3 * HI + H] = (torch.randn(3 * HI + H, D, device = 'cuda', generator = g) / D ** 0.5).to(BF16)
-    gq, gk = (torch.randn(64, device = 'cuda', generator = g) * 0.3 for _ in range(2))
-    pos = torch.randint(0, 900, (M,), device = 'cuda', generator = g, dtype = torch.int32)
-    freqs, t, tt = _rope_tables(ops, 1024)
-    q, k, v = (torch.zeros(M, HI, device = 'cuda', dtype = BF16) for _ in range(3))
-    gates = torch.zeros(M, H, device = 'cuda'); inv = torch.zeros(M, 2 * H, device = 'cuda')
-    ops.gemm_qkvg(u, D, W, D, M, H, D, q, k, v, gates, inv, gq, gk, pos, tt, 1024, None, None)
-    y = u.float() @ W.float().t()
-    rms = lambda x, gm: torch.nn.functional.normalize(x, dim = -1) * 8. * (gm + 1.)
-    qr = _rope_ref(rms(y[:, :HI].reshape(M, H, 64), gq), pos, freqs).reshape(M, HI)
-    kr = _rope_ref(rms(y[:, HI:2 * HI].reshape(M, H, 64), gk), pos, freqs).reshape(M, HI)
-    torch.cuda.synchronize()
-    assert torch.allclose(q.float(), qr, atol = 6e-2, rtol = 2e-2) and torch.allclose(k.float(), kr, atol = 6e-2, rtol = 2e-2)
-    assert torch.allclose(v.float(), y[:, 2 * HI:3 * HI], atol = 3e-2, rtol = 2e-2)
-    assert torch.allclose(gates, y[:, 3 * HI:3 * HI + H], atol = 2e-2, rtol = 1e-2)
-    want_inv = 1. / y[:, :2 * HI].reshape(M, 2 * H, 64).norm(dim = -1)
-    assert torch.allclose(inv, want_inv, rtol = 1e-2, atol = 1e-4)
-    # kv-cache append: k / v rows land at kv_rows[m] of a larger matrix, q stays dense
-    rows = torch.randperm(2 * M + 50, device = 'cuda', generator = g)[:M].to(torch.int32)
-    kc = torch.zeros(2 * M + 50, HI, device = 'cuda', dtype = BF16); vc = torch.zeros_like(kc)
-    q2 = torch.zeros_like(q)
-    ops.gemm_qkvg(u, D, W, D, M, H, D, q2, kc, vc, gates, inv, gq, gk, pos, tt, 1024, rows, None)
-    torch.cuda.synchronize()
-    assert torch.equal(q2, q) and torch.equal(kc[rows.long()], k) and torch.equal(vc[rows.long()], v)
-    untouched = torch.ones(2 * M + 50, dtype = torch.bool, device = 'cuda'); untouched[rows.long()] = False
-    assert (kc[untouched] == 0).all() and (vc[untouched] == 0).all()
-
-
-@pytest.mark.parametrize('M,N,K,two', [(900, 512, 512, False), (333, 512, 1408, False), (500, 512, 1024, True), (130, 128, 128, False)])
-def test_gemm_resid_epilogue_vs_torch(ops, cluster_mode, M, N, K, two):
-    """branch output projection + AdaptiveWrapper output gate + residual (T.py:765-769, 1031, 1238-1242); `two`: skip_proj on cat(x, skip) (T.py:1217-1219)"""
-    g = torch.Generator(device = 'cuda').manual_seed(5)
-    nc = 4
-    A = torch.randn(M, K, device = 'cuda', generator = g).to(BF16)
-    W = (torch.randn(N, K, device = 'cuda', generator = g) / K ** 0.5).to(BF16)
-    bias = torch.randn(N, device = 'cuda', generator = g) * 0.2
-    x_res = torch.randn(M, N, device = 'cuda', generator = g)
-    x_out = torch.zeros(M, N, device = 'cuda'); xb = torch.zeros(M, N, device = 'cuda', dtype = BF16); yb = torch.zeros(M, N, device = 'cuda', dtype = BF16)
-    y = A.float() @ W.float().t()
-    if two:
-        A1, A2 = A[:, :K // 2].contiguous(), A[:, K // 2:].contiguous()
-        ops.gemm_resid(A1, K // 2, A2, K // 2, K // 2, W, K, M, N, K, None, x_res, x_out, xb, None, None, None, 0, None)
-        torch.cuda.synchronize()
-        want = x_res + y
-        assert torch.allclose(x_out, want, atol = 3e-2, rtol = 1e-2) and torch.allclose(xb.float(), want, atol = 6e-2, rtol = 2e-2)
-        return
-    cond_row = torch.randint(-1, nc, (M,), device = 'cuda', generator = g, dtype = torch.int32)
-    zg = torch.rand(nc, 3 * N, device = 'cuda', generator = g)                       # strided table: row pitch 3N, this wrapper's slice starts at column N
-    ls = torch.randn(N, device = 'cuda', generator = g) * 0.3
-    ops.gemm_resid(A, K, None, 0, 0, W, K, M, N, K, bias, x_res, x_out, None, yb, cond_row, zg[:, N:], 3 * N, ls)
-    torch.cuda.synchronize()
-    yy = y + bias
-    cr = cond_row.long().clamp(min = 0)
-    scale = torch.where((cond_row >= 0)[:, None], zg[cr, N:2 * N], ls + 1.)
-    assert torch.allclose(yb.float(), yy, atol = 6e-2, rtol = 2e-2)
-    assert torch.allclose(x_out, x_res + yy * scale, atol = 4e-2, rtol = 1e-2)
-    # text-only form (no condition table): layerscale on every row
-    ops.gemm_resid(A, K, None, 0, 0, W, K, M, N, K, bias, x_res, x_out, None, None, None, None, 0, ls)
-    torch.cuda.synchronize()
-    assert torch.allclose(x_out, x_res + yy * (ls + 1.), atol = 4e-2, rtol = 1e-2)
-
-
-@pytest.mark.parametrize('M,D,inner', [(600, 512, 1365), (200, 128, 341)])
-def test_gemm_geglu_epilogue_and_backward_vs_torch(ops, cluster_mode, M, D, inner):
-    """FeedForward net.0 + GEGLU (T.py:833-834, 846-847) on the tile-interleaved W1, and tfx_geglu_bwd against autograd"""
-    g = torch.Generator(device = 'cuda').manual_seed(6)
-    Ip = (inner + 63) // 64 * 64
-    W1 = torch.randn(2 * inner, D, device = 'cuda', generator = g) / D ** 0.5          # rows [value 0..inner) | gate inner..2 inner)  (T.py:833)
-    b1 = torch.randn(2 * inner, device = 'cuda', generator = g) * 0.3
-    u = torch.randn(M, D, device = 'cuda', generator = g).to(BF16)
-    Wp = torch.zeros(2 * Ip, D, device = 'cuda'); bp = torch.zeros(2 * Ip, device = 'cuda')
-    col = torch.arange(Ip, device = 'cuda')
-    valid = col < inner
-    tile, j = col // 64, col % 64
-    Wp[(tile * 128 + j)[valid]] = W1[col[valid]]; Wp[(tile * 128 + 64 + j)[valid]] = W1[inner + col[valid]]
-    bp[(tile * 128 + j)[valid]] = b1[col[valid]]; bp[(tile * 128 + 64 + j)[valid]] = b1[inner + col[valid]]
-    Wp = Wp.to(BF16)
-    vg = torch.zeros(M, 2 * Ip, device = 'cuda', dtype = BF16); h = torch.zeros(M, Ip, device = 'cuda', dtype = BF16)
-    ops.gemm_geglu(u, D, Wp, D, bp, M, 2 * Ip, D, vg, h)
-    pre = u.float() @ W1.to(BF16).float().t() + b1
-    val, gate = pre[:, :inner], pre[:, inner:]
-    want_h = torch.nn.functional.gelu(gate) * val
-    torch.cuda.synchronize()
-    assert torch.allclose(h[:, :inner].float(), want_h, atol = 6e-2, rtol = 3e-2) and (h[:, inner:] == 0).all()
-    got_val = vg.float().reshape(M, Ip // 64, 2, 64)[:, :, 0].reshape(M, Ip)[:, :inner]
-    got_gate = vg.float().reshape(M, Ip // 64, 2, 64)[:, :, 1].reshape(M, Ip)[:, :inner]
-    assert torch.allclose(got_val, val, atol = 6e-2, rtol = 2e-2) and torch.allclose(got_gate, gate, atol = 6e-2, rtol = 2e-2)
-    # backward from the SAVED bf16 pre-activations
-    dh = torch.zeros(M, Ip, device = 'cuda', dtype = BF16)
-    dh[:, :inner] = torch.randn(M, inner, device = 'cuda', generator = g).to(BF16)
-    dvg = torch.zeros_like(vg)
-    rpb = ops.lib.tfx_geglu_bwd_rows_per_block()
-    nblk = (M + rpb - 1) // rpb
-    part = torch.zeros(nblk, 2 * Ip, device = 'cuda')
-    ops.geglu_bwd(dh, vg, dvg, M, Ip, None, None, part)
-    vgf = vg.float().reshape(M, Ip // 64, 2, 64)
-    v_s, g_s = vgf[:, :, 0].reshape(M, Ip).clone().requires_grad_(True), vgf[:, :, 1].reshape(M, Ip).clone().requires_grad_(True)
-    (torch.nn.functional.gelu(g_s) * v_s).backward(dh.float())
-    torch.cuda.synchronize()
-    dv_got = dvg.float().reshape(M, Ip // 64, 2, 64)[:, :, 0].reshape(M, Ip)
-    dg_got = dvg.float().reshape(M, Ip // 64, 2, 64)[:, :, 1].reshape(M, Ip)
-    assert torch.allclose(dv_got, v_s.grad, atol = 3e-2, rtol = 2e-2) and torch.allclose(dg_got, g_s.grad, atol = 3e-2, rtol = 2e-2)
-    colsum = part.sum(0).reshape(Ip // 64, 2, 64)
-    assert torch.allclose(colsum[:, 0].reshape(Ip), dvg.float().reshape(M, Ip // 64, 2, 64)[:, :, 0].reshape(M, Ip).sum(0), atol = 0.5, rtol = 2e-2)
-    assert torch.allclose(colsum[:, 1].reshape(Ip), dg_got.sum(0), atol = 0.5, rtol = 2e-2)
-
-
 # ================================================================================================ backward row kernels vs autograd
 def test_adaln_and_resid_backward_vs_autograd(ops):
     M, D, nc = 1500, 512, 6
@@ -381,21 +252,6 @@ def test_adaln_and_resid_backward_vs_autograd(ops):
     torch.cuda.synchronize()
     assert torch.allclose(dx - 0.25, x.grad, atol = 2e-3, rtol = 2e-3)
     assert torch.allclose(dfilm, film.grad, atol = 2e-2, rtol = 2e-3) and torch.allclose(dgam, gam.grad, atol = 2e-2, rtol = 2e-3)
-    # ---- output gate backward: x_out = x_res + y * s,  s = isM ? zgate[cr] : layerscale + 1
-    y = torch.randn(M, D, device = 'cuda', generator = g).to(BF16)
-    zg = torch.rand(nc, 3 * D, device = 'cuda', generator = g).requires_grad_(True)
-    ls = (torch.randn(D, device = 'cuda', generator = g) * 0.3).requires_grad_(True)
-    yf = y.float().requires_grad_(True)
-    s = torch.where(isM, zg[cr, D:2 * D], ls + 1.)
-    dxo = torch.randn(M, D, device = 'cuda', generator = g)
-    (yf * s).backward(dxo)
-    dy = torch.zeros(M, D, device = 'cuda', dtype = BF16)
-    dzg = torch.zeros(nc, 3 * D, device = 'cuda'); dls = torch.zeros(D, device = 'cuda'); dbias = torch.zeros(D, device = 'cuda')
-    ops.resid_bwd(dxo, y, cond_row, zg.detach()[:, D:], 3 * D, ls.detach(), dy, dzg[:, D:], 3 * D, dls, dbias, M, D)
-    torch.cuda.synchronize()
-    assert torch.allclose(dy.float(), yf.grad, atol = 3e-2, rtol = 2e-2)
-    assert torch.allclose(dzg, zg.grad, atol = 3e-2, rtol = 3e-3) and torch.allclose(dls, ls.grad, atol = 3e-2, rtol = 3e-3)
-    assert torch.allclose(dbias, dy.float().sum(0), atol = 0.2, rtol = 1e-2)
 
 
 def test_attn_residual_rmsnorm_embed_backward_vs_autograd(ops):
@@ -458,36 +314,6 @@ def test_attn_residual_rmsnorm_embed_backward_vs_autograd(ops):
     torch.cuda.synchronize()
     assert torch.allclose(demb, want_emb, atol = 1e-3, rtol = 1e-4)
     assert torch.allclose(dmod.float(), dx0[rows], atol = 3e-2, rtol = 1e-2)
-
-
-def test_qk_bwd_pack_vs_autograd(ops):
-    """backward of the qk-RMSNorm + RoPE epilogue (T.py:950-965) and of the value gate logits (T.py:1026-1027)"""
-    M, H = 640, 4
-    HI, NQ = H * 64, 3 * H * 64 + 128
-    g = torch.Generator(device = 'cuda').manual_seed(9)
-    freqs, t, tt = _rope_tables(ops, 1024)
-    pos = torch.randint(0, 900, (M,), device = 'cuda', generator = g, dtype = torch.int32)
-    xq = torch.randn(M, H, 64, device = 'cuda', generator = g).requires_grad_(True)
-    xk = torch.randn(M, H, 64, device = 'cuda', generator = g).requires_grad_(True)
-    gq = (torch.randn(64, device = 'cuda', generator = g) * 0.3).requires_grad_(True)
-    gk = (torch.randn(64, device = 'cuda', generator = g) * 0.3).requires_grad_(True)
-    rms = lambda x, gm: torch.nn.functional.normalize(x, dim = -1) * 8. * (gm + 1.)
-    q = _rope_ref(rms(xq, gq), pos, freqs); k = _rope_ref(rms(xk, gk), pos, freqs)
-    dq = torch.randn(M, HI, device = 'cuda', generator = g); dk = torch.randn(M, HI, device = 'cuda', generator = g)
-    (q.reshape(M, HI) * dq).sum().backward(retain_graph = True)
-    (k.reshape(M, HI) * dk).sum().backward()
-    inv = torch.cat((1. / xq.detach().norm(dim = -1), 1. / xk.detach().norm(dim = -1)), dim = 1).contiguous()          # [M, 2H]
-    gates = torch.randn(M, H, device = 'cuda', generator = g)
-    dsum = torch.randn(M, H, device = 'cuda', generator = g)
-    out = torch.zeros(M, NQ, device = 'cuda', dtype = BF16)
-    dgq = torch.zeros(64, device = 'cuda'); dgk = torch.zeros(64, device = 'cuda')
-    ops.qk_bwd_pack(dq, dk, q.detach().reshape(M, HI).to(BF16), k.detach().reshape(M, HI).to(BF16), inv, gq.detach(), gk.detach(), pos, t, gates, dsum, out, NQ, dgq, dgk, M, H)
-    torch.cuda.synchronize()
-    # the kernel reconstructs xhat from the bf16 q / k it is given: tolerances are those of bf16 inputs
-    assert torch.allclose(out[:, :HI].float(), xq.grad.reshape(M, HI), atol = 8e-2, rtol = 5e-2)
-    assert torch.allclose(out[:, HI:2 * HI].float(), xk.grad.reshape(M, HI), atol = 8e-2, rtol = 5e-2)
-    assert torch.allclose(out[:, 3 * HI:3 * HI + H].float(), (1 - torch.sigmoid(gates)) * dsum, atol = 2e-2, rtol = 2e-2)
-    assert torch.allclose(dgq, gq.grad, atol = 0.5, rtol = 3e-2) and torch.allclose(dgk, gk.grad, atol = 0.5, rtol = 3e-2)
 
 
 # ================================================================================================ decode-path kernels

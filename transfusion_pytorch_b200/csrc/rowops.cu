@@ -808,6 +808,9 @@ __global__ void __launch_bounds__(ROW_THREADS) clean_flow_bwd_k(float* __restric
 // forward (GEMM epilogue): xhat = x*inv;  y = xhat*8*(gamma+1);  q = R(pos) y (interleaved pairs)   (T.py:950-965)
 // One warp per token; 8 lanes share a head (lane owns 8 consecutive dims = 4 rope pairs: 32 B fp32 / 16 B bf16 accesses),
 // so a warp covers 4 heads per pass and the per-head dot product is a 3-step shuffle.
+// xhat is rebuilt from the bf16 output as R^T q / (8 (gamma + 1)): where gamma_j = -1 the forward wrote y_j = 0 and xhat_j is lost, so
+// dx_j and dgamma_j come out 0 instead of -inv xhat_j (xhat . dxhat) and sum 8 dy_j xhat_j; near -1 the bf16 error of the rope partner is
+// amplified by |gamma_partner + 1| / |gamma_j + 1|.
 __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_k(const float* __restrict__ dq, const float* __restrict__ dk, const __nv_bfloat16* __restrict__ q,
                                                             const __nv_bfloat16* __restrict__ k, const float* __restrict__ qk_inv, const float* __restrict__ gq,
                                                             const float* __restrict__ gk, const int* __restrict__ rope_pos, const float2* __restrict__ rope_cs,
