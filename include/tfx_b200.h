@@ -153,22 +153,13 @@ int tfx_adaln_bwd(const float* du, const float* x, const float* stats, const int
  * dbias (optional, [D]) += column sums of dy (gradient of the bias of the producing Linear, T.py:849) */
 int tfx_resid_bwd(const float* dx, const void* y_bf16, const int* cond_row, const float* zgate, long long zgate_ld, const float* layerscale,
                   void* dy_bf16, float* dzgate, long long dzgate_ld, float* dlayerscale, float* dbias, int M, int D, void* stream);
-/* AttentionResidual (T.py:803-829): softmax mix over all hiddens so far, single pass; lse_out [M] (optional) = log-sum-exp of the
- * depth softmax, consumed by the backward together with the forward output x_out so that every hidden is read exactly once.
- * 1 <= n_hiddens <= TFX_MAX_DEPTH + 1 (forward and accumulating backward). */
-int tfx_attn_residual_fwd(const float* const* hiddens, int n_hiddens, const float* gamma, const float* pseudo_query,
-                          float* x_out, void* x_out_bf16, float* lse_out, int M, int D, void* stream);
-long long tfx_attn_residual_bwd_workspace_floats(int M, int D);   /* fp32 scratch for the per-block parameter-gradient partial sums */
-int tfx_attn_residual_bwd(const float* const* hiddens, float* const* dhiddens, int n_hiddens, const float* gamma, const float* pseudo_query,
-                          const float* dx_out, const float* x_out, const float* lse, float* dgamma, float* dpseudo_query, float* workspace, int M, int D,
-                          int init /* 1: dhiddens are overwritten, not accumulated */, void* stream);
-/* same two kernels reading bf16 COPIES of the hiddens (engine option hid_bf16: the AttentionResidual read traffic - the largest HBM term of the step - halves;
- * gradients w.r.t. the hiddens stay fp32) */
+/* AttentionResidual forward (T.py:803-829): softmax mix over all hiddens so far, single pass.  The hiddens are bf16 (the layer outputs are kept
+ * in bf16 only: reading them is the largest HBM term of the step); x_out fp32, x_out_bf16 (optional) its bf16 copy.  lse_out [M] (optional) =
+ * log-sum-exp of the depth softmax, consumed by the backward (tfx_attn_residual_bwd2) together with x_out so that every hidden is read once per layer.
+ * 1 <= n_hiddens <= TFX_MAX_DEPTH + 1. */
 int tfx_attn_residual_fwd_h16(const void* const* hiddens_bf16, int n_hiddens, const float* gamma, const float* pseudo_query,
                               float* x_out, void* x_out_bf16, float* lse_out, int M, int D, void* stream);
-int tfx_attn_residual_bwd_h16(const void* const* hiddens_bf16, float* const* dhiddens, int n_hiddens, const float* gamma, const float* pseudo_query,
-                              const float* dx_out, const float* x_out, const float* lse, float* dgamma, float* dpseudo_query, float* workspace, int M, int D, int init,
-                              void* stream);
+long long tfx_attn_residual_bwd_workspace_floats(int M, int D);   /* fp32 scratch of tfx_attn_residual_bwd2 for the per-block parameter-gradient partial sums */
 /* final RMSNorm (T.py:1250, 785-786) (+ compaction of modality rows for the flow head) */
 int tfx_rmsnorm_fwd(const float* x, const float* gamma, float* out_f32, void* out_bf16, const int* slot, void* out_mod_bf16, int M, int D, void* stream);
 int tfx_rmsnorm_bwd(const float* dout, const float* x, const float* gamma, float* dx, float* dgamma, int M, int D, void* stream);

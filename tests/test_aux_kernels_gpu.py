@@ -1,5 +1,5 @@
-"""GPU: the kernels around the block stack - loss, conditioning, bias gradients, weight repack, optimizer step, token / flow path,
-AttentionResidual with bf16 hiddens and the RoPE table - each called through the C ABI and compared with a float64 restatement of its formula.
+"""GPU: the kernels around the block stack - loss, conditioning, bias gradients, weight repack, optimizer step, token / flow path
+and the RoPE table - each called through the C ABI and compared with a float64 restatement of its formula.
 
 Tolerances:
   - copies and casts are compared bit for bit (int16 / int32 views); torch's fp32 -> bf16 cast rounds to nearest even, like the kernels;
@@ -11,7 +11,6 @@ Tolerances:
 Shapes are large enough for every grid-stride / multi-row loop to run more than once: element-wise kernels cap their grid at
 num_SMs x 16 blocks of 256 threads (n >= 4M), the warp-per-row kernels at num_SMs x 8 blocks of 8 warps (rows > 8448), CE at num_SMs x 64 warps.
 Bytes a kernel must not touch (padding columns, skipped rows, a guard row past the end) hold a sentinel and are checked unchanged."""
-import ctypes
 import math
 
 import numpy as np
@@ -635,53 +634,6 @@ def test_embed_scatter_clean_flow(ops, D):
     assert torch.equal(dneg[:S], -dmod[:S])
     assert not dmod[:S][~ok].any() and not dneg[:S][~ok].any(), 'skipped rows get a zero gradient'
     assert same_bits(dmod[S], dm0[S]) and (dneg[S] == 5.).all()
-
-
-# ------------------------------------------------------------------------------------------------ AttentionResidual, bf16 hiddens
-def _parr(ts):
-    arr = (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
-    return arr, ctypes.cast(arr, ctypes.c_void_p)
-
-
-@pytest.mark.parametrize('D', [128, 512, 1024])
-def test_attn_residual_bwd_h16(ops, D):
-    M, L1 = 900, 5
-    g = gen(30 + D)
-    hid16 = [torch.randn(M, D, device = 'cuda', generator = g).to(BF16) for _ in range(L1)]
-    hid = [h.double().requires_grad_(True) for h in hid16]           # fp64 autograd on the bf16-rounded hiddens
-    gam = (torch.randn(D, device = 'cuda', generator = g) * 0.3)
-    pq = (torch.randn(D, device = 'cuda', generator = g) * 0.5)
-    gam64, pq64 = gam.double().requires_grad_(True), pq.double().requires_grad_(True)
-    vals = torch.stack(hid)
-    keys = torch.nn.functional.normalize(vals, dim = -1) * D ** 0.5 * (gam64 + 1)
-    sim = torch.einsum('lnd,d->nl', keys, pq64) * D ** -0.5
-    want = torch.einsum('nl,lnd->nd', sim.softmax(-1), vals)
-    dxo = torch.randn(M, D, device = 'cuda', generator = g)
-    want.backward(dxo.double())
-    k16, p16 = _parr(hid16)
-    xo = torch.zeros(M, D, device = 'cuda'); lse = torch.zeros(M, device = 'cuda')
-    ops.attn_residual_fwd_h16(p16, L1, gam, pq, xo, None, lse, M, D)
-    ws = torch.zeros(int(ops.lib.tfx_attn_residual_bwd_workspace_floats(M, D)), device = 'cuda')
-    dh = [torch.full((M, D), 0.5, device = 'cuda') for _ in range(L1)]
-    kd, pd = _parr(dh)
-    dgam = torch.zeros(D, device = 'cuda'); dpq = torch.zeros(D, device = 'cuda')
-    ops.attn_residual_bwd_h16(p16, pd, L1, gam, pq, dxo, xo, lse, dgam, dpq, ws, M, D, 0)
-    assert torch.allclose(xo.double(), want.detach(), atol = 1e-4, rtol = 1e-4)
-    for l in range(L1):
-        assert torch.allclose((dh[l] - 0.5).double(), hid[l].grad, atol = 2e-4, rtol = 2e-3), ('init 0 accumulates', l)
-    assert torch.allclose(dgam.double(), gam64.grad, atol = 2e-3, rtol = 5e-3) and torch.allclose(dpq.double(), pq64.grad, atol = 2e-3, rtol = 5e-3)
-    ops.attn_residual_bwd_h16(p16, pd, L1, gam, pq, dxo, xo, lse, dgam, dpq, ws, M, D, 1)
-    for l in range(L1):
-        assert torch.allclose(dh[l].double(), hid[l].grad, atol = 2e-4, rtol = 2e-3), ('init 1 overwrites', l)
-    # the fp32-hidden kernel on the same (bf16-representable) values agrees to fp32 rounding
-    h32 = [h.float() for h in hid16]
-    k32, p32 = _parr(h32)
-    dh32 = [torch.zeros(M, D, device = 'cuda') for _ in range(L1)]
-    kd32, pd32 = _parr(dh32)
-    dgam32 = torch.zeros(D, device = 'cuda'); dpq32 = torch.zeros(D, device = 'cuda')
-    ops.attn_residual_bwd(p32, pd32, L1, gam, pq, dxo, xo, lse, dgam32, dpq32, ws, M, D, 1)
-    for l in range(L1):
-        assert torch.allclose(dh[l], dh32[l], atol = 1e-6, rtol = 1e-5), l
 
 
 # ------------------------------------------------------------------------------------------------ RoPE table

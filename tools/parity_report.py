@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Prints, per reference-generated fixture, the relative error of the loss / breakdown and the worst hidden-state and gradient-fingerprint errors of the
-CUDA path (the numbers the parity tests bound).  Run once per engine option, e.g.  TFX_HIDDEN_BF16=1 python tools/parity_report.py"""
+CUDA path (the numbers the parity tests bound).  Run once per engine option, e.g.  TFX_GEMM_CLUSTER=2 python tools/parity_report.py"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))

@@ -37,11 +37,8 @@ SIGNATURES = {
     'tfx_adaln_fwd': [VP, VP, VP, LL, VP, VP, VP, I, I, VP],
     'tfx_adaln_bwd': [VP, VP, VP, VP, VP, LL, VP, VP, VP, LL, VP, I, I, VP],
     'tfx_resid_bwd': [VP, VP, VP, VP, LL, VP, VP, VP, LL, VP, VP, I, I, VP],
-    'tfx_attn_residual_fwd': [VP, I, VP, VP, VP, VP, VP, I, I, VP],
-    'tfx_attn_residual_bwd': [VP, VP, I, VP, VP, VP, VP, VP, VP, VP, VP, I, I, I, VP],
     'tfx_attn_residual_bwd2': [VP, I, I, VP, VP, VP, VP, I, VP, VP, VP, VP, VP, I, VP, VP, VP, I, I, VP],
     'tfx_attn_residual_fwd_h16': [VP, I, VP, VP, VP, VP, VP, I, I, VP],
-    'tfx_attn_residual_bwd_h16': [VP, VP, I, VP, VP, VP, VP, VP, VP, VP, VP, I, I, I, VP],
     'tfx_rmsnorm_fwd': [VP, VP, VP, VP, VP, VP, I, I, VP],
     'tfx_rmsnorm_bwd': [VP, VP, VP, VP, VP, I, I, VP],
     'tfx_rep_cos_fwd_bwd': [VP, VP, I, VP, I, VP, VP, VP, VP, I, I, VP],

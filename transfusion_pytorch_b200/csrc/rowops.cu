@@ -11,7 +11,7 @@
 namespace tfx {
 
 constexpr int MAX_HIDDENS = TFX_MAX_DEPTH + 1;    // x0 and every layer output: 65 pointers, 520 B of kernel parameters
-struct PtrList { float* p[MAX_HIDDENS]; };
+struct HiddenList { const __nv_bfloat16* p[MAX_HIDDENS]; };
 
 // ------------------------------------------------------------------------------------ adaLN forward
 // u = isM ? LN(x)*(gamma_c+1)+beta_c : LN(x)*(g+1)      (T.py:747-755; text-only 677-679)
@@ -243,12 +243,12 @@ __global__ void __launch_bounds__(ROW_THREADS) resid_bwd_k(const float* __restri
 // filled by lane-private cp.async pieces: RING - 1 row loads per warp stay in flight without spending registers (a register double buffer
 // would need twice the registers per row and halve the resident warps).
 constexpr int ARES_FWD_RING = 4;
-template <int NCH, bool HB>
-__global__ void __launch_bounds__(ROW_THREADS) attn_res_fwd_k(PtrList hid, int L1, const float* __restrict__ gamma, const float* __restrict__ pq,
+template <int NCH>
+__global__ void __launch_bounds__(ROW_THREADS) attn_res_fwd_k(HiddenList hid, int L1, const float* __restrict__ gamma, const float* __restrict__ pq,
                                                              float* __restrict__ xo, __nv_bfloat16* __restrict__ xb, float* __restrict__ lse_out, int M) {
   constexpr int D = NCH * 128;
   constexpr int RING = ARES_FWD_RING;
-  constexpr int SLOT = D * (HB ? 2 : 4);
+  constexpr int SLOT = D * 2;                                   // bytes: one bf16 row
   const int lane = threadIdx.x & 31;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   extern __shared__ __align__(16) uint8_t ares_ring[];
@@ -258,15 +258,9 @@ __global__ void __launch_bounds__(ROW_THREADS) attn_res_fwd_k(PtrList hid, int L
   auto issue = [&]() {
     if (iss_row < M) {
       const uint32_t dst = ring_u32 + iss_slot * SLOT;
-      if (HB) {
-        const __nv_bfloat16* b = reinterpret_cast<const __nv_bfloat16*>(hid.p[iss_k]) + (long long)iss_row * D + lane * 4;
+      const __nv_bfloat16* b = hid.p[iss_k] + (long long)iss_row * D + lane * 4;
 #pragma unroll
-        for (int c = 0; c < NCH; ++c) cp_async_8(dst + (c * 128 + lane * 4) * 2, b + c * 128);
-      } else {
-        const float* f = hid.p[iss_k] + (long long)iss_row * D + lane * 4;
-#pragma unroll
-        for (int c = 0; c < NCH; ++c) cp_async_16(dst + (c * 128 + lane * 4) * 4, f + c * 128);
-      }
+      for (int c = 0; c < NCH; ++c) cp_async_8(dst + (c * 128 + lane * 4) * 2, b + c * 128);
       if (++iss_k == L1) { iss_k = 0; iss_row += nwarps; }
     }
     cp_async_commit();
@@ -288,8 +282,7 @@ __global__ void __launch_bounds__(ROW_THREADS) attn_res_fwd_k(PtrList hid, int L
     for (int k = 0; k < L1; ++k) {
       float h[NCH * 4];
       cp_async_wait<RING - 1>();
-      if (HB) load_row_bf16<NCH>(reinterpret_cast<const __nv_bfloat16*>(ring + cons_slot * SLOT), lane, h);
-      else load_row_f32<NCH>(reinterpret_cast<const float*>(ring + cons_slot * SLOT), lane, h);
+      load_row_bf16<NCH>(reinterpret_cast<const __nv_bfloat16*>(ring + cons_slot * SLOT), lane, h);
       cons_slot = cons_slot + 1 == RING ? 0 : cons_slot + 1;
       issue();
       float ss = 0.f, dot = 0.f;
@@ -314,92 +307,17 @@ __global__ void __launch_bounds__(ROW_THREADS) attn_res_fwd_k(PtrList hid, int L
   cp_async_wait<0>();
 }
 
-// ------------------------------------------------------------------------------------ AttentionResidual backward
-// dh_l += alpha_l*dx + dsim_l*(w/|h| - <h,w> h/|h|^3);   dw += dsim_l*h/|h|   (dw -> d gamma, d pq)
-// Single pass over the hiddens: alpha_l = exp(sim_l - lse) uses the log-sum-exp saved by the forward, and the softmax-backward
-// mean  sum_k alpha_k <h_k, dx>  equals <x_out, dx> (x_out is the saved forward output) - so every h_l is read exactly once.
-template <int NCH, bool HB>
-__global__ void __launch_bounds__(ROW_THREADS, 2) attn_res_bwd_k(PtrList hid, PtrList dhid, int L1, const float* __restrict__ gamma, const float* __restrict__ pq,
-                                                                const float* __restrict__ dxo, const float* __restrict__ xo, const float* __restrict__ lse,
-                                                                float* __restrict__ partials, int M, int tpw, int init) {
-  constexpr int D = NCH * 128;
-  const int lane = threadIdx.x & 31;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);    // (no early return: block-wide barriers below)
-  __shared__ __align__(16) float w_s[D];             // w = (gamma+1) * pq, shared by the block (keeps 16 registers free)
-  for (int c = threadIdx.x; c < D; c += ROW_THREADS) w_s[c] = (gamma[c] + 1.f) * pq[c];
-  __syncthreads();
-  float accw[NCH * 4];
-#pragma unroll
-  for (int i = 0; i < NCH * 4; ++i) accw[i] = 0.f;
-  for (int row = r0; row < r1; ++row) {
-    float dxv[NCH * 4], h[NCH * 4];
-    load_row_f32<NCH>(dxo + (long long)row * D, lane, dxv);
-    load_row_f32<NCH>(xo + (long long)row * D, lane, h);
-    float mean_da = 0.f;
-#pragma unroll
-    for (int i = 0; i < NCH * 4; ++i) mean_da += h[i] * dxv[i];
-    mean_da = warp_sum(mean_da);
-    const float lse_r = lse[row];
-    if (HB) load_row_bf16<NCH>(reinterpret_cast<const __nv_bfloat16*>(hid.p[0]) + (long long)row * D, lane, h);
-    else load_row_f32<NCH>(hid.p[0] + (long long)row * D, lane, h);
-    for (int k = 0; k < L1; ++k) {
-      float hn[NCH * 4], g[NCH * 4];
-      if (k + 1 < L1) {                                                                    // prefetch the next hidden
-        if (HB) load_row_bf16<NCH>(reinterpret_cast<const __nv_bfloat16*>(hid.p[k + 1]) + (long long)row * D, lane, hn);
-        else load_row_f32<NCH>(hid.p[k + 1] + (long long)row * D, lane, hn);
-      }
-      if (!init) load_row_f32<NCH>(dhid.p[k] + (long long)row * D, lane, g);
-      else {
-#pragma unroll
-        for (int i = 0; i < NCH * 4; ++i) g[i] = 0.f;
-      }
-      float w[NCH * 4];
-      load_row_f32<NCH>(w_s, lane, w);
-      float ss = 0.f, dot = 0.f, da = 0.f;
-#pragma unroll
-      for (int i = 0; i < NCH * 4; ++i) { ss += h[i] * h[i]; dot += h[i] * w[i]; da += h[i] * dxv[i]; }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        ss += __shfl_xor_sync(0xffffffffu, ss, o); dot += __shfl_xor_sync(0xffffffffu, dot, o); da += __shfl_xor_sync(0xffffffffu, da, o);
-      }
-      const float nrm = fmaxf(sqrtf(ss), 1e-12f), rn = 1.f / nrm;
-      const float a = __expf(dot * rn - lse_r);
-      const float ds = a * (da - mean_da);
-      const float c1 = ds * rn, c2 = ds * dot * rn * rn * rn;
-#pragma unroll
-      for (int i = 0; i < NCH * 4; ++i) {
-        g[i] += a * dxv[i] + c1 * w[i] - c2 * h[i];
-        accw[i] += c1 * h[i];
-      }
-      store_row_f32<NCH>(dhid.p[k] + (long long)row * D, lane, g);
-      if (k + 1 < L1) {
-#pragma unroll
-        for (int i = 0; i < NCH * 4; ++i) h[i] = hn[i];
-      }
-    }
-  }
-  // d w = sum over tokens of c1 * h: block-level reduction, then ONE row of partial sums per block (no same-address atomics from
-  // thousands of warps); attn_res_bwd_finish_k folds the partials into d gamma = dw * pq and d pq = dw * (gamma + 1)
-  __shared__ float red[WARPS_PER_BLOCK][D];
-  store_row_f32<NCH>(red[threadIdx.x >> 5], lane, accw);
-  __syncthreads();
-  for (int c = threadIdx.x; c < D; c += ROW_THREADS) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < WARPS_PER_BLOCK; ++w) t += red[w][c];
-    partials[(long long)blockIdx.x * D + c] = t;
-  }
-}
-
-// ------------------------------------------------------------------------------------ AttentionResidual backward, DEFERRED assembly (exact, less traffic)
-// The accumulating version above adds  a_k dx + c1_k w - c2_k h_k  into dH_k for EVERY earlier hidden k at EVERY layer: a read-modify-write of (i + 2)
-// fp32 rows per token and layer (68 % of that kernel's bytes).  Each contribution is (per-token scalars) x (a vector that already exists: the incoming
-// gradient dx_i', the layer's w_i', the hidden itself), so this version stores the three scalars per (token, layer, hidden) - 12 bytes instead of 2 KB -
-// and assembles the COMPLETE gradient of one hidden, once, when the backward pass needs it:
+// ------------------------------------------------------------------------------------ AttentionResidual backward, deferred assembly
+// Layer i' adds to the gradient of every hidden k it mixes  a_k dx + c1_k w - c2_k h_k,  and to dw (-> d gamma, d pq)  c1_k h_k, where
+//     a_k = exp(sim_k - lse)  (the log-sum-exp saved by the forward),   ds_k = a_k (<h_k, dx> - <x_out, dx>),   c1_k = ds_k / |h_k|,   c2_k = ds_k <h_k, w> / |h_k|^3
+// (the softmax-backward mean  sum_k a_k <h_k, dx>  equals <x_out, dx>, x_out being the saved forward output, so every h_k is read once per layer).
+// Adding these terms into dH_k at every layer would read-modify-write (i + 2) fp32 rows per token and layer.  Each term is (per-token scalars) x (a vector
+// that already exists: the incoming gradient dx_i', the layer's w_i', the hidden itself), so this kernel stores the three scalars per (token, layer, hidden) -
+// 12 bytes instead of 2 KB - and assembles the COMPLETE gradient of one hidden, once, when the backward pass needs it:
 //     G_k = sum_{i' >= k-1} [ a_{i',k} dx_{i'} + c1_{i',k} w_{i'} ] - (sum_{i'} c2_{i',k}) h_k
 // Layer i (own = 1): scalar pass over h_0 .. h_{i+1} (parameter gradients, scalars out), then G_{i+1} from its own term and the stored scalars / incoming
-// gradients of the later layers.  own = 0: only the assembly (G_0, after the first layer).  Bytes per token over 8 layers: 167 KB instead of 234 KB.
+// gradients of the later layers.  own = 0: only the assembly (G_0, after the first layer).  Bytes per token over 8 layers: 167 KB instead of the 234 KB of
+// accumulating into dH_k at every layer.
 // One launch assembles at most BWD2_CHUNK later layers (their w rows in shared memory, one lane each for their scalars).  The sum is linear in the
 // later layers, so deeper models add the rest chunk by chunk: ACC launches (own = 0) add their chunk's terms, c2 part included, into G.
 constexpr int BWD2_CHUNK = 10;
@@ -960,70 +878,30 @@ int tfx_resid_bwd(const float* dx, const void* y_bf16, const int* cond_row, cons
   return check_launch("resid_bwd");
 }
 
-static int attn_residual_fwd_impl(const void* const* hiddens, bool hb, int n_hiddens, const float* gamma, const float* pseudo_query,
-                                  float* x_out, void* x_out_bf16, float* lse_out, int M, int D, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(n_hiddens >= 1 && n_hiddens <= MAX_HIDDENS, "attn_residual: n_hiddens %d out of range [1,%d]", n_hiddens, MAX_HIDDENS);
-  PtrList pl;
-  for (int i = 0; i < n_hiddens; ++i) pl.p[i] = reinterpret_cast<float*>(const_cast<void*>(hiddens[i]));
-  // persistent grid: exactly the resident blocks (registers / ring shared memory decide), rows strided over all warps
-#define TFX_ARES_FWD_LAUNCH(HBV)                                                                                                            \
-  TFX_DISPATCH_NCH(D, {                                                                                                                     \
-    auto kern = attn_res_fwd_k<NCH, HBV>;                                                                                                   \
-    const int smem = WARPS_PER_BLOCK * ARES_FWD_RING * D * (HBV ? 2 : 4);                                                                   \
-    static int per_sm = 0;                                                                                                                  \
-    if (!per_sm) {                                                                                                                          \
-      cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);                                                        \
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, ROW_THREADS, smem);                                                      \
-      if (per_sm < 1) per_sm = 1;                                                                                                           \
-    }                                                                                                                                       \
-    const long long want = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, cap = (long long)num_sms() * per_sm;                     \
-    kern<<<(int)(want < cap ? want : cap), ROW_THREADS, smem, ST(stream)>>>(pl, n_hiddens, gamma, pseudo_query, x_out, (__nv_bfloat16*)x_out_bf16, lse_out, M); \
-  })
-  if (hb) TFX_ARES_FWD_LAUNCH(true); else TFX_ARES_FWD_LAUNCH(false);
-#undef TFX_ARES_FWD_LAUNCH
-  return check_launch("attn_residual_fwd");
-}
-int tfx_attn_residual_fwd(const float* const* hiddens, int n_hiddens, const float* gamma, const float* pseudo_query,
-                          float* x_out, void* x_out_bf16, float* lse_out, int M, int D, void* stream) {
-  return attn_residual_fwd_impl(reinterpret_cast<const void* const*>(hiddens), false, n_hiddens, gamma, pseudo_query, x_out, x_out_bf16, lse_out, M, D, stream);
-}
 int tfx_attn_residual_fwd_h16(const void* const* hiddens_bf16, int n_hiddens, const float* gamma, const float* pseudo_query,
                               float* x_out, void* x_out_bf16, float* lse_out, int M, int D, void* stream) {
-  return attn_residual_fwd_impl(hiddens_bf16, true, n_hiddens, gamma, pseudo_query, x_out, x_out_bf16, lse_out, M, D, stream);
-}
-
-static const int ATTN_RES_BWD_TPW = 4;
-static const int ATTN_RES_BWD2_TPW = 8;      // the ring start-up bubble is paid once per warp: more rows per warp (the workspace is sized for the smaller constant)
-long long tfx_attn_residual_bwd_workspace_floats(int M, int D) { return (long long)chunk_grid(M, ATTN_RES_BWD_TPW) * D; }
-
-static int attn_residual_bwd_impl(const void* const* hiddens, bool hb, float* const* dhiddens, int n_hiddens, const float* gamma, const float* pseudo_query,
-                                  const float* dx_out, const float* x_out, const float* lse, float* dgamma, float* dpseudo_query, float* workspace, int M, int D, int init,
-                                  void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(n_hiddens >= 1 && n_hiddens <= MAX_HIDDENS, "attn_residual: n_hiddens %d out of range [1,%d]", n_hiddens, MAX_HIDDENS);
-  TFX_REQUIRE(workspace != nullptr, "attn_residual_bwd: workspace of tfx_attn_residual_bwd_workspace_floats(M, D) floats is required");
-  PtrList pl, dl;
-  for (int i = 0; i < n_hiddens; ++i) { pl.p[i] = reinterpret_cast<float*>(const_cast<void*>(hiddens[i])); dl.p[i] = dhiddens[i]; }
-  const int tpw = ATTN_RES_BWD_TPW;
-  const int blocks = chunk_grid(M, tpw);
-  if (hb) TFX_DISPATCH_NCH(D, (attn_res_bwd_k<NCH, true><<<blocks, ROW_THREADS, 0, ST(stream)>>>(pl, dl, n_hiddens, gamma, pseudo_query, dx_out, x_out, lse, workspace, M, tpw, init)));
-  else TFX_DISPATCH_NCH(D, (attn_res_bwd_k<NCH, false><<<blocks, ROW_THREADS, 0, ST(stream)>>>(pl, dl, n_hiddens, gamma, pseudo_query, dx_out, x_out, lse, workspace, M, tpw, init)));
-  if (int rc = check_launch("attn_residual_bwd")) return rc;
-  const int rpb = 16;
-  attn_res_bwd_finish_k<<<dim3((D + 127) / 128, (blocks + rpb - 1) / rpb), 128, 0, ST(stream)>>>(workspace, blocks, D, gamma, pseudo_query, dgamma, dpseudo_query, rpb);
-  return check_launch("attn_residual_bwd_finish");
+  HiddenList hl;
+  for (int i = 0; i < n_hiddens; ++i) hl.p[i] = reinterpret_cast<const __nv_bfloat16*>(hiddens_bf16[i]);
+  // persistent grid: exactly the resident blocks (registers / ring shared memory decide), rows strided over all warps
+  TFX_DISPATCH_NCH(D, {
+    auto kern = attn_res_fwd_k<NCH>;
+    const int smem = WARPS_PER_BLOCK * ARES_FWD_RING * D * 2;
+    static int per_sm = 0;
+    if (!per_sm) {
+      cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, ROW_THREADS, smem);
+      if (per_sm < 1) per_sm = 1;
+    }
+    const long long want = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, cap = (long long)num_sms() * per_sm;
+    kern<<<(int)(want < cap ? want : cap), ROW_THREADS, smem, ST(stream)>>>(hl, n_hiddens, gamma, pseudo_query, x_out, (__nv_bfloat16*)x_out_bf16, lse_out, M);
+  });
+  return check_launch("attn_residual_fwd");
 }
-int tfx_attn_residual_bwd(const float* const* hiddens, float* const* dhiddens, int n_hiddens, const float* gamma, const float* pseudo_query,
-                          const float* dx_out, const float* x_out, const float* lse, float* dgamma, float* dpseudo_query, float* workspace, int M, int D, int init,
-                          void* stream) {
-  return attn_residual_bwd_impl(reinterpret_cast<const void* const*>(hiddens), false, dhiddens, n_hiddens, gamma, pseudo_query, dx_out, x_out, lse, dgamma, dpseudo_query, workspace, M, D, init, stream);
-}
-int tfx_attn_residual_bwd_h16(const void* const* hiddens_bf16, float* const* dhiddens, int n_hiddens, const float* gamma, const float* pseudo_query,
-                              const float* dx_out, const float* x_out, const float* lse, float* dgamma, float* dpseudo_query, float* workspace, int M, int D, int init,
-                              void* stream) {
-  return attn_residual_bwd_impl(hiddens_bf16, true, dhiddens, n_hiddens, gamma, pseudo_query, dx_out, x_out, lse, dgamma, dpseudo_query, workspace, M, D, init, stream);
-}
+
+static const int ATTN_RES_BWD2_TPW = 8;      // the ring start-up bubble is paid once per warp: more rows per warp
+long long tfx_attn_residual_bwd_workspace_floats(int M, int D) { return (long long)chunk_grid(M, ATTN_RES_BWD2_TPW) * D; }
 
 int tfx_attn_residual_bwd2(const void* const* hiddens_bf16, int n_hiddens, int own, const float* const* gammas, const float* const* pseudo_queries,
                            const float* const* dx_later, const float* const* scalars_later, int n_later, const float* dx_out, const float* x_out, const float* lse,

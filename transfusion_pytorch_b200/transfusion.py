@@ -575,7 +575,7 @@ class Transfusion(SamplingMixin, Module):
             for b in range(rb.B):
                 out[b, :rb.seq_lens[b]] = t[rb.cu[b]:rb.cu[b + 1]]
             return out
-        return [unpack(h.float().clone()) for h in (*st['hid'], st['out'])]      # (bf16 copies when the engine runs with hid_bf16)
+        return [unpack(h.float().clone()) for h in (*st['hid'], st['out'])]      # (the engine keeps the layer hiddens in bf16)
 
     @torch.no_grad()
     def generate_text_only(self, prompt: Tensor, seq_len: int, temperature = 1.0, min_p = 0.1, cache_kv = True, seed = None, use_cuda_graph = True) -> Tensor:
