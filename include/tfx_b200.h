@@ -142,7 +142,7 @@ int tfx_vmix_bwd(void* dv_inout, long long ld_dv, const void* v_mixed, long long
                  float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream);
 int tfx_add_f32_into_bf16(void* dst_bf16, long long ld_dst, const float* src, long long ld_src, int M, int N, void* stream);
 
-/* ---------------------------------------------------------------- warp-per-token kernels (D = model dim, multiple of 128, <= 1024)
+/* ---------------------------------------------------------------- warp-per-token kernels (D = model dim: 128, 256, 384, 512, 768 or 1024)
  * AdaptiveWrapper input side (T.py:747-755, text-only 677-679): u = isM ? LN(x)(gamma_c+1)+beta_c : LN(x)(g+1).
  * film points at [n_cond][film_ld] with gamma at +0 and beta at +D; cond_row NULL = all text.      */
 int tfx_adaln_fwd(const float* x, const int* cond_row, const float* film, long long film_ld, const float* ln_gamma,

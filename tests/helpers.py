@@ -1,11 +1,76 @@
-"""Shared helpers of the parity tests: rebuild the exact inputs the golden fixtures were generated from."""
+"""Shared helpers of the tests: rebuild the exact inputs the golden fixtures were generated from (parity tests), and the comparison /
+sentinel plumbing of the float64 kernel tests (Checks, guarded outputs, bit-exact untouched checks, the GEMM cluster-mode fixture)."""
 import os
 
+import numpy as np
+import pytest
 import torch
 
 from transfusion_pytorch_b200 import synth
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
+BF16, F32 = torch.bfloat16, torch.float32
+SENT = -77.5                          # exact in bf16 and fp32
+
+
+# ------------------------------------------------------------------------------------------------ float64 kernel tests
+class Checks:
+    """collects every comparison of a test, prints its worst err / bound and fails at the end with all the violations.
+    `shown`: the calling module's dict of worst err / bound per check name, printed at the end of the module."""
+
+    def __init__(self, what, shown):
+        self.what, self.shown, self.bad = what, shown, []
+
+    def __call__(self, name, got, ref, bound):
+        got = got.double()
+        err = (got - ref).abs()
+        ratio = (err / bound.clamp_min(1e-300)).nan_to_num(nan = float('inf'))
+        r = ratio.max().item() if ratio.numel() else 0.
+        self.shown[name] = max(self.shown.get(name, 0.), r)
+        print(f'{self.what} {name}: worst err / bound {r:.3g}')
+        if not torch.isfinite(got).all():
+            self.bad.append(f'{name}: non-finite values')
+        elif r > 1:
+            i = np.unravel_index(int(ratio.argmax()), tuple(ratio.shape))
+            self.bad.append(f'{name}: {int((ratio > 1).sum())} values off, worst err / bound {r:.3e} at {tuple(int(x) for x in i)} '
+                            f'(got {got[i].item():.6e}, ref {ref[i].item():.6e})')
+
+    def true(self, name, ok):
+        if not ok:
+            self.bad.append(name)
+
+    def done(self):
+        assert not self.bad, f'{self.what}:\n  ' + '\n  '.join(self.bad)
+
+
+def gen(seed):
+    return torch.Generator(device = 'cuda').manual_seed(seed)
+
+
+def guarded(rows, cols, dtype):
+    """a sentinel-filled [rows + 1, cols] buffer and its first `rows` rows; the last row is a guard the kernel must not touch"""
+    buf = torch.full((rows + 1, cols), SENT, device = 'cuda', dtype = dtype)
+    return buf, buf[:rows]
+
+
+def same_bits(a, b):
+    view = {BF16: torch.int16, F32: torch.int32}
+    return torch.equal(a.contiguous().view(view[a.dtype]), b.contiguous().view(view[b.dtype]))
+
+
+def untouched(t):
+    return same_bits(t, torch.full_like(t, SENT))
+
+
+@pytest.fixture(params = [1, 2], ids = ['single', 'paired'])
+def cluster_mode(ops, request):
+    """GEMM launches as independent CTAs (default) and as 2-CTA clusters sharing the B tile by TMA multicast"""
+    assert ops.lib.tfx_gemm_set_cluster_mode(request.param) == 0
+    yield request.param
+    ops.lib.tfx_gemm_set_cluster_mode(1)
+
+
+# ------------------------------------------------------------------------------------------------ parity tests
 
 
 def load_golden(name):

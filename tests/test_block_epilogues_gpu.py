@@ -31,13 +31,13 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import SENT, Checks as _Checks, cluster_mode, gen, guarded, same_bits, untouched  # noqa: F401  (cluster_mode: a fixture)
 from transfusion_pytorch_b200 import _lib, engine as E
 from oracle.dropout_mask import keep_mask, scale as drop_scale, SITE_FFN
 
 pytestmark = pytest.mark.gpu
 BF16, F32, F64, I32 = torch.bfloat16, torch.float32, torch.float64, torch.int32
 U8, U24 = 2.0 ** -8, 2.0 ** -24       # bf16 cast, one fp32 rounding (relative)
-SENT = -77.5                          # exact in bf16 and fp32
 M_ROWS = 9011
 N_POS = 16384                         # RoPE table length; positions run to its last entry
 ZERO_ROW = 4321                       # an all-zero row of u in the QKVG test
@@ -61,14 +61,6 @@ def ops():
     return _lib.Ops()
 
 
-@pytest.fixture(params = [1, 2], ids = ['single', 'paired'])
-def cluster_mode(ops, request):
-    """GEMM launches as independent CTAs (default) and as 2-CTA clusters sharing the B tile by TMA multicast"""
-    assert ops.lib.tfx_gemm_set_cluster_mode(request.param) == 0
-    yield request.param
-    ops.lib.tfx_gemm_set_cluster_mode(1)
-
-
 SHOWN = {}
 
 
@@ -79,51 +71,8 @@ def _report():
         print(f'worst over the file: {name:28s} {r:.3g}')
 
 
-class Checks:
-    """collects every comparison of a test, prints its worst err / bound and fails at the end with all the violations"""
-
-    def __init__(self, what):
-        self.what, self.bad = what, []
-
-    def __call__(self, name, got, ref, bound):
-        got = got.double()
-        err = (got - ref).abs()
-        ratio = (err / bound.clamp_min(1e-300)).nan_to_num(nan = float('inf'))
-        r = ratio.max().item() if ratio.numel() else 0.
-        SHOWN[name] = max(SHOWN.get(name, 0.), r)
-        print(f'{self.what} {name}: worst err / bound {r:.3g}')
-        if not torch.isfinite(got).all():
-            self.bad.append(f'{name}: non-finite values')
-        elif r > 1:
-            i = np.unravel_index(int(ratio.argmax()), tuple(ratio.shape))
-            self.bad.append(f'{name}: {int((ratio > 1).sum())} values off, worst err / bound {r:.3e} at {tuple(int(x) for x in i)} '
-                            f'(got {got[i].item():.6e}, ref {ref[i].item():.6e})')
-
-    def true(self, name, ok):
-        if not ok:
-            self.bad.append(name)
-
-    def done(self):
-        assert not self.bad, f'{self.what}:\n  ' + '\n  '.join(self.bad)
-
-
-def gen(seed):
-    return torch.Generator(device = 'cuda').manual_seed(seed)
-
-
-def guarded(rows, cols, dtype):
-    """a sentinel-filled [rows + 1, cols] buffer and its first `rows` rows; the last row is a guard the kernel must not touch"""
-    buf = torch.full((rows + 1, cols), SENT, device = 'cuda', dtype = dtype)
-    return buf, buf[:rows]
-
-
-def same_bits(a, b):
-    view = {BF16: torch.int16, F32: torch.int32}
-    return torch.equal(a.contiguous().view(view[a.dtype]), b.contiguous().view(view[b.dtype]))
-
-
-def untouched(t):
-    return same_bits(t, torch.full_like(t, SENT))
+def Checks(what):
+    return _Checks(what, SHOWN)
 
 
 def gemm64(a, w):

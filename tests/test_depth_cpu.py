@@ -10,7 +10,7 @@ from helpers import load_golden, golden_noise
 from oracle.make_golden_deep import INTERLEAVED, deep_batch
 from test_oracle_cpu import REL, build, check_grads
 from transfusion_pytorch_b200 import Transfusion, synth
-from transfusion_pytorch_b200.transfusion import MAX_DEPTH, Transformer
+from transfusion_pytorch_b200.transfusion import MAX_DEPTH, MODEL_DIMS, Transformer
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -63,3 +63,27 @@ def test_depth_limit():
         Transformer(128, depth = 65, heads = 2)
     with pytest.raises(NotImplementedError, match = 'depth'):
         Transfusion(num_text_tokens = 16, transformer = dict(dim = 128, depth = 65, heads = 2))
+
+
+def test_width_and_head_limits():
+    """the accepted widths are the widths the row kernels dispatch (the case labels of TFX_DISPATCH_NCH, D = 128 * NCH) and the widths the
+    README lists; other widths and head counts the attention kernels do not take are rejected where the model is built"""
+    with open(os.path.join(ROOT, 'transfusion_pytorch_b200', 'csrc', 'common.cuh')) as f:
+        src = f.read()
+    macro = src[src.index('#define TFX_DISPATCH_NCH'):]
+    macro = macro[:macro.index('} while (0)')]
+    dispatched = {128 * int(n) for n in re.findall(r'case (\d+):', macro)}
+    assert dispatched == set(MODEL_DIMS) and len(MODEL_DIMS) == len(dispatched)
+    with open(os.path.join(ROOT, 'README.md')) as f:
+        line = re.search(r'width \(`dim`\) ([\d, or]+) with', f.read()).group(1)
+    assert {int(w) for w in re.findall(r'\d+', line)} == set(MODEL_DIMS)
+    for D in MODEL_DIMS:
+        Transformer(D, depth = 1, heads = 2)
+    Transformer(128, depth = 1, heads = 32)
+    with pytest.raises(NotImplementedError, match = 'dim 640'):
+        Transformer(640, depth = 2, heads = 2)
+    with pytest.raises(NotImplementedError, match = 'dim 896'):
+        Transformer(896, depth = 2, heads = 2)
+    for heads in (3, 34, 0):
+        with pytest.raises(NotImplementedError, match = f'heads {heads} '):
+            Transformer(128, depth = 2, heads = heads)

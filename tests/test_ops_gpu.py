@@ -17,41 +17,6 @@ def ops():
     return _lib.Ops()
 
 
-@pytest.fixture(params = [1, 2], ids = ['single', 'paired'])
-def cluster_mode(ops, request):
-    """GEMM launches as independent CTAs (default) and as 2-CTA clusters sharing the B tile by TMA multicast"""
-    assert ops.lib.tfx_gemm_set_cluster_mode(request.param) == 0
-    yield request.param
-    ops.lib.tfx_gemm_set_cluster_mode(1)
-
-
-@pytest.mark.parametrize('a_mn,b_mn', [(0, 0), (0, 1), (1, 1), (1, 0)])
-@pytest.mark.parametrize('M,N,K', [(300, 390, 520), (1000, 1664, 512), (128, 128, 64), (40000, 512, 192)])      # the last one: several tiles per CTA (pair), odd tile count
-def test_gemm_store_all_majors(ops, cluster_mode, a_mn, b_mn, M, N, K):
-    g = torch.Generator(device = 'cuda').manual_seed(0)
-    A = torch.randn(M, K, device = 'cuda', generator = g).to(BF16)
-    B = torch.randn(N, K, device = 'cuda', generator = g).to(BF16)
-    ref = A.float() @ B.float().t()
-    pad8 = lambda x: (x + 7) // 8 * 8
-    def store(mat, mn):                      # mat is [MN, K]; returns (tensor, ld)
-        if mn:
-            t = torch.zeros(K, pad8(mat.shape[0]), device = 'cuda', dtype = BF16); t[:, :mat.shape[0]] = mat.t(); return t, t.shape[1]
-        t = torch.zeros(mat.shape[0], pad8(K), device = 'cuda', dtype = BF16); t[:, :K] = mat; return t, t.shape[1]
-    (a, lda), (b, ldb) = store(A, a_mn), store(B, b_mn)
-    out = torch.zeros(M, N, device = 'cuda', dtype = F32)
-    outb = torch.zeros(M, pad8(N), device = 'cuda', dtype = BF16)
-    bias = torch.randn(N, device = 'cuda')
-    ops.gemm_store(a, lda, a_mn, b, ldb, b_mn, M, N, K, out, N, outb, pad8(N), bias, None, 0.5, 0, 1)
-    torch.cuda.synchronize()
-    want = 0.5 * ref + bias
-    assert torch.allclose(out, want, atol = 2e-2, rtol = 1e-3)
-    assert torch.allclose(outb[:, :N].float(), want, atol = 0.15, rtol = 2e-2)
-    acc = torch.ones(M, N, device = 'cuda', dtype = F32)
-    ops.gemm_store(a, lda, a_mn, b, ldb, b_mn, M, N, K, acc, N, None, 0, None, None, 1.0, 1, 4)
-    torch.cuda.synchronize()
-    assert torch.allclose(acc, ref + 1, atol = 2e-2, rtol = 1e-3)
-
-
 def dense_attention(q, k, v, gates, kv_limit, cu, scale, cap):
     out = torch.zeros_like(q, dtype = F32)
     H = q.shape[1] // 64
@@ -184,22 +149,6 @@ def test_attention_tcgen05_fast_path_vs_dense(ops, lens, spans):
     assert fp[0].item() == 0.0
 
 
-def test_adaln_fwd_vs_torch(ops):
-    M, D, nc = 777, 512, 5
-    g = torch.Generator(device = 'cuda').manual_seed(2)
-    x = torch.randn(M, D, device = 'cuda', generator = g) * 3 + 1
-    cond_row = torch.randint(-1, nc, (M,), device = 'cuda', generator = g, dtype = torch.int32)
-    film = torch.randn(nc, 2 * D, device = 'cuda', generator = g) * 0.3
-    gam = torch.randn(D, device = 'cuda', generator = g) * 0.3
-    u = torch.zeros(M, D, device = 'cuda', dtype = BF16); stats = torch.zeros(M, 2, device = 'cuda')
-    ops.adaln_fwd(x, cond_row, film, 2 * D, gam, u, stats, M, D)
-    xh = torch.nn.functional.layer_norm(x, (D,))
-    cr = cond_row.long().clamp(min = 0)
-    want = torch.where((cond_row >= 0)[:, None], xh * (film[cr, :D] + 1) + film[cr, D:], xh * (gam + 1))
-    torch.cuda.synchronize()
-    assert torch.allclose(u.float(), want, atol = 3e-2, rtol = 1e-2)
-
-
 def test_ce_and_mse_heads_vs_torch(ops):
     M, V = 500, 390
     g = torch.Generator(device = 'cuda').manual_seed(3)
@@ -213,65 +162,6 @@ def test_ce_and_mse_heads_vs_torch(ops):
     torch.cuda.synchronize()
     assert abs(acc.item() - ref.item()) / ref.item() < 1e-5 and nv.item() == int((labels >= 0).sum())
     assert torch.allclose(dl[:, :V].float(), lg.grad, atol = 2e-3, rtol = 1e-2) and (dl[:, V:] == 0).all()
-
-
-# ================================================================================================ backward row kernels vs autograd
-def test_adaln_and_resid_backward_vs_autograd(ops):
-    M, D, nc = 1500, 512, 6
-    g = torch.Generator(device = 'cuda').manual_seed(7)
-    x = (torch.randn(M, D, device = 'cuda', generator = g) * 2 + 0.5).requires_grad_(True)
-    cond_row = torch.sort(torch.randint(-1, nc, (M,), device = 'cuda', generator = g, dtype = torch.int32)).values          # runs of equal rows, as in a packed batch
-    cond_row = cond_row[torch.randperm(30, device = 'cuda', generator = g).repeat_interleave(50)[:M].argsort(stable = True)]   # ... in shuffled chunks
-    W3 = 7 * D
-    film = (torch.randn(nc, W3, device = 'cuda', generator = g) * 0.3).requires_grad_(True)                                   # strided table, this wrapper at column D
-    gam = (torch.randn(D, device = 'cuda', generator = g) * 0.3).requires_grad_(True)
-    u = torch.zeros(M, D, device = 'cuda', dtype = BF16); stats = torch.zeros(M, 2, device = 'cuda')
-    ops.adaln_fwd(x.detach(), cond_row, film.detach()[:, D:], W3, gam.detach(), u, stats, M, D)
-    isM = (cond_row >= 0)[:, None]
-    cr = cond_row.long().clamp(min = 0)
-    xh = torch.nn.functional.layer_norm(x, (D,))
-    want_u = torch.where(isM, xh * (film[cr, D:2 * D] + 1) + film[cr, 2 * D:3 * D], xh * (gam + 1))
-    du = torch.randn(M, D, device = 'cuda', generator = g)
-    want_u.backward(du)
-    dx = torch.full((M, D), 0.25, device = 'cuda')                      # accumulated into
-    dfilm = torch.zeros(nc, W3, device = 'cuda'); dgam = torch.zeros(D, device = 'cuda')
-    ops.adaln_bwd(du, x.detach(), stats, cond_row, film.detach()[:, D:], W3, gam.detach(), dx, dfilm[:, D:], W3, dgam, M, D)
-    torch.cuda.synchronize()
-    assert torch.allclose(dx - 0.25, x.grad, atol = 2e-3, rtol = 2e-3)
-    assert torch.allclose(dfilm, film.grad, atol = 2e-2, rtol = 2e-3) and torch.allclose(dgam, gam.grad, atol = 2e-2, rtol = 2e-3)
-
-
-def test_rmsnorm_embed_backward_vs_autograd(ops):
-    M, D = 900, 512
-    g = torch.Generator(device = 'cuda').manual_seed(8)
-    # ---- final RMSNorm
-    x = (torch.randn(M, D, device = 'cuda', generator = g) * 1.5).requires_grad_(True)
-    gn = (torch.randn(D, device = 'cuda', generator = g) * 0.3).requires_grad_(True)
-    out = torch.nn.functional.normalize(x, dim = -1) * D ** 0.5 * (gn + 1)
-    dout = torch.randn(M, D, device = 'cuda', generator = g)
-    out.backward(dout)
-    of = torch.zeros(M, D, device = 'cuda'); ob = torch.zeros(M, D, device = 'cuda', dtype = BF16)
-    ops.rmsnorm_fwd(x.detach(), gn.detach(), of, ob, None, None, M, D)
-    dx = torch.zeros(M, D, device = 'cuda'); dgn = torch.zeros(D, device = 'cuda')
-    ops.rmsnorm_bwd(dout, x.detach(), gn.detach(), dx, dgn, M, D)
-    torch.cuda.synchronize()
-    assert torch.allclose(of, out.detach(), atol = 1e-4, rtol = 1e-4)
-    assert torch.allclose(dx, x.grad, atol = 2e-4, rtol = 2e-3) and torch.allclose(dgn, gn.grad, atol = 5e-3, rtol = 5e-3)
-    # ---- token assemble backward: text rows scatter-add into the embedding gradient, modality rows go to the compact matrix
-    V, S = 70, 300
-    text_id = torch.randint(0, V, (M,), device = 'cuda', generator = g, dtype = torch.int32)
-    slot = torch.full((M,), -1, device = 'cuda', dtype = torch.int32)
-    rows = torch.randperm(M, device = 'cuda', generator = g)[:S]
-    slot[rows] = torch.arange(S, device = 'cuda', dtype = torch.int32)
-    dx0 = torch.randn(M, D, device = 'cuda', generator = g)
-    demb = torch.zeros(V, D, device = 'cuda'); dmod = torch.zeros(S, D, device = 'cuda', dtype = BF16)
-    ops.embed_bwd(dx0, text_id, slot, demb, dmod, M, D)
-    want_emb = torch.zeros(V, D, device = 'cuda')
-    is_text = slot < 0
-    want_emb.index_add_(0, text_id[is_text].long(), dx0[is_text])
-    torch.cuda.synchronize()
-    assert torch.allclose(demb, want_emb, atol = 1e-3, rtol = 1e-4)
-    assert torch.allclose(dmod.float(), dx0[rows], atol = 3e-2, rtol = 1e-2)
 
 
 # ================================================================================================ decode-path kernels

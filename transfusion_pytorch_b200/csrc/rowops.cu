@@ -561,7 +561,8 @@ __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_bwd_k(const float* __rest
     float ss = 0.f;
 #pragma unroll
     for (int i = 0; i < NCH * 4; ++i) ss += v[i] * v[i];
-    const float rn = 1.f / fmaxf(sqrtf(warp_sum(ss)), 1e-12f);
+    const float nrm = sqrtf(warp_sum(ss));
+    const float rn = 1.f / fmaxf(nrm, 1e-12f);
     float dot = 0.f;
 #pragma unroll
     for (int i = 0; i < NCH * 4; ++i) {
@@ -571,6 +572,7 @@ __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_bwd_k(const float* __rest
       dot += d[i] * v[i];
     }
     dot = warp_sum(dot);
+    if (nrm < 1e-12f) dot = 0.f;               // clamped norm: a constant for the gradient (F.normalize), dx = d xhat / eps
 #pragma unroll
     for (int i = 0; i < NCH * 4; ++i) d[i] = rn * (d[i] - v[i] * dot);
     store_row_f32<NCH>(dx + (long long)row * D, lane, d);

@@ -30,6 +30,7 @@ from torch import Tensor
 from . import _lib
 from ._pinned import POOL
 from .modality_processing import RaggedBatch
+from .transfusion import MODEL_DIMS, MIN_HEADS, MAX_HEADS
 
 BF16, F32, I32, I64 = torch.bfloat16, torch.float32, torch.int32, torch.int64
 
@@ -163,8 +164,8 @@ class Engine:
         self.scale = 64 ** -0.5
         self.dls = list(model.dim_latents)
         self.dlp = [_round_up(d, 8) for d in self.dls]
-        assert self.D % 128 == 0 and self.D <= 1024, 'model dim must be a multiple of 128 and <= 1024 for the row kernels'
-        assert self.H % 2 == 0 and 2 <= self.H <= 32, 'heads must be even (two 64-wide heads per 128-column GEMM tile)'
+        assert self.D in MODEL_DIMS, f'model dim must be one of {MODEL_DIMS} for the row kernels'
+        assert self.H % 2 == 0 and MIN_HEADS <= self.H <= MAX_HEADS, 'heads must be even (two 64-wide heads per 128-column GEMM tile) and at most 32'
         self.device = None
         self.flat = None
         self.ws = {}

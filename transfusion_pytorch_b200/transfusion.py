@@ -29,6 +29,10 @@ from .modality_processing import (
 
 # Deepest model the AttentionResidual kernels take (TFX_MAX_DEPTH in include/tfx_b200.h): their hidden-state lists hold x0 and 64 layer outputs
 MAX_DEPTH = 64
+# Model widths the row kernels are built for: the cases of TFX_DISPATCH_NCH (csrc/common.cuh), D = 128 * NCH
+MODEL_DIMS = (128, 256, 384, 512, 768, 1024)
+# Heads the attention kernels take: two 64-wide heads per 128-column GEMM tile, at most 32 (gemm_qkvg's 32-column gate slab)
+MIN_HEADS, MAX_HEADS = 2, 32
 
 
 class TextKVCache:
@@ -208,6 +212,8 @@ class Transformer(Module):
         unsupported = []
         if dim_head != 64: unsupported.append('dim_head != 64')
         if depth > MAX_DEPTH: unsupported.append(f'depth {depth} > {MAX_DEPTH}')
+        if dim not in MODEL_DIMS: unsupported.append(f'dim {dim} (the row kernels take {", ".join(map(str, MODEL_DIMS))})')
+        if heads % 2 or not MIN_HEADS <= heads <= MAX_HEADS: unsupported.append(f'heads {heads} (must be even and in [{MIN_HEADS}, {MAX_HEADS}])')
         ff_dropout = float(ff_kwargs.get('dropout', 0.))
         for name, p in (('dropout', dropout), ("ff_kwargs['dropout']", ff_dropout)):
             if not 0. <= p <= 1.:
