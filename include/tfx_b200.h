@@ -254,7 +254,9 @@ int tfx_attn_decode(const void* q, const void* k, const void* v, long long ld_q,
                     const int* tile_q0, const int* tile_kv0, const int* tile_kvend, int n_tiles, void* o, long long ld_o, float scale, float softcap, void* stream);
 /* token sampling + state update for every sample in the text phase (sample_text_token T.py:580-591; greedy / gumbel of generate_text_only
  * T.py:2692-2698 with vlimit = num_text_tokens; bookkeeping T.py:2330-2349).  rows (optional): logits row of sample s (first token after the
- * prefill, taken at the last prompt position, T.py:2225-2250: advance = 0 - that token only gets its cache row on the next step). */
+ * prefill, taken at the last prompt position, T.py:2225-2250: advance = 0 - that token only gets its cache row on the next step).
+ * Tempered draw of sample s: argmax over the kept ids c of logit / T - log(-log u), u = ((h >> 41) + 1/2) 2^-23 with
+ * h = mix64(seed ^ mix64((counters[1] << 40) ^ (s << 20) ^ c)) (splitmix64 finaliser; counters NULL: step 0). */
 int tfx_sample_tokens(const float* logits, long long ld_logits, const int* rows, int V, int vlimit, int* state, int S, int* hist, int hist_cap, int eos_id, const int* som_ids,
                       int n_som, int max_length, float temperature, float min_p, unsigned long long seed, int* counters, int advance, void* stream);
 /* fixed-grid explicit midpoint (torchdiffeq method='midpoint', T.py:1314-1318, 2523-2525) on device state; tab [n_evals][4] = (t, c, h, mode), *idx = the

@@ -164,112 +164,6 @@ def test_ce_and_mse_heads_vs_torch(ops):
     assert torch.allclose(dl[:, :V].float(), lg.grad, atol = 2e-3, rtol = 1e-2) and (dl[:, V:] == 0).all()
 
 
-# ================================================================================================ decode-path kernels
-def test_attn_decode_vs_dense(ops):
-    """single-query decode attention over cache slabs (csrc/decode.cu) against the dense formula, incl. slabs of very different fill"""
-    H, cap_rows, S = 4, 700, 5
-    scale, softcap = 0.125, 50.
-    g = torch.Generator(device = 'cuda').manual_seed(10)
-    lens = [1, 33, 128, 300, 699]
-    kc = (torch.randn(S * cap_rows, H * 64, device = 'cuda', generator = g) * 1.5).to(BF16); vc = (torch.randn(S * cap_rows, H * 64, device = 'cuda', generator = g) * 2).to(BF16)
-    q = (torch.randn(S, H * 64, device = 'cuda', generator = g) * 1.5).to(BF16)
-    gates = torch.randn(S, H, device = 'cuda', generator = g)
-    i32 = lambda v: torch.tensor(v, device = 'cuda', dtype = torch.int32)
-    kv0 = i32([s * cap_rows for s in range(S)]); kvend = i32([s * cap_rows + lens[s] for s in range(S)])
-    lim = kvend - 1
-    o = torch.zeros(S, H * 64, device = 'cuda', dtype = BF16)
-    ops.attn_decode(q, kc, vc, H * 64, H * 64, H * 64, gates, H, lim, i32(list(range(S))), kv0, kvend, S, o, H * 64, scale, softcap)
-    torch.cuda.synchronize()
-    for s in range(S):
-        kk = kc[s * cap_rows: s * cap_rows + lens[s]].float().reshape(lens[s], H, 64)
-        vv = vc[s * cap_rows: s * cap_rows + lens[s]].float().reshape(lens[s], H, 64)
-        sim = torch.einsum('hd,jhd->hj', q[s].float().reshape(H, 64) * scale, kk)
-        sim = torch.tanh(sim / softcap) * softcap
-        want = torch.einsum('hj,jhd->hd', sim.softmax(-1), vv) * torch.sigmoid(gates[s])[:, None]
-        assert torch.allclose(o[s].float().reshape(H, 64), want, atol = 3e-2, rtol = 3e-2), s
-
-
-def test_sample_tokens_and_decode_prep(ops):
-    """tfx_sample_tokens: greedy = torch.argmax; min-p + Gumbel draws follow the filtered softmax; the state machine of T.py:2330-2349.
-    tfx_decode_prep: state -> metadata of the next text step."""
-    S, V, ld = 64, 390, 392
-    g = torch.Generator(device = 'cuda').manual_seed(11)
-    logits = torch.randn(S, ld, device = 'cuda', generator = g) * 2
-    st = torch.zeros(6, S, device = 'cuda', dtype = torch.int32)
-    st[0] = 10; st[1] = 7
-    st[3, 5] = 2; st[3, 6] = 1                                          # one finished sample, one waiting for its modality: untouched
-    hist = torch.zeros(S, 8, device = 'cuda', dtype = torch.int32); cnt = torch.zeros(2, device = 'cuda', dtype = torch.int32)
-    som = torch.tensor([259], device = 'cuda', dtype = torch.int32)
-    logits[3, 257] = 50.; logits[4, 259] = 50.                          # sample 3 draws [eos], sample 4 draws [som]
-    before = st.clone()
-    ops.sample_tokens(logits, ld, None, V, 0, st, S, hist, 8, 257, som, 1, 1000, 0.0, 0.1, 1234, cnt, 1)
-    torch.cuda.synchronize()
-    want = logits[:, :V].argmax(-1).int()
-    act = torch.ones(S, dtype = torch.bool, device = 'cuda'); act[5] = act[6] = False
-    assert torch.equal(st[2][act], want[act]) and torch.equal(hist[:, 0][act], want[act]) and torch.equal(st[:, ~act], before[:, ~act])
-    assert (st[0][act] == 11).all() and (st[1][act] == 8).all() and (st[4][act] == 1).all() and (st[5][act] == 1).all()
-    assert st[3, 3].item() == 2 and st[3, 4].item() == 1 and cnt[0].item() == int(act.sum()) - 2
-    # length limit: num_tokens > max_length ends the sample
-    st2 = torch.zeros(6, S, device = 'cuda', dtype = torch.int32); st2[4] = 5
-    ops.sample_tokens(logits, ld, None, V, 0, st2, S, hist, 8, -1, som, 0, 5, 0.0, 0.1, 1, cnt, 0)
-    torch.cuda.synchronize()
-    assert (st2[3] == 2).all() and (st2[0] == 0).all() and (st2[1] == 0).all()          # advance = 0: first token after the prefill
-    # Gumbel-max draws: empirical frequencies over many (sample, step) pairs follow softmax(min-p filtered logits / T), restricted to ids < vlimit
-    Vs, T, minp = 12, 0.7, 0.2
-    base = torch.tensor([2.0, 1.5, 1.0, 0.0, -1.0, -3.0, 0.5, 1.8, -0.5, 0.2, 3.0, 2.5], device = 'cuda')
-    lg = torch.zeros(4096, 16, device = 'cuda'); lg[:, :Vs] = base
-    counts = torch.zeros(Vs, device = 'cuda')
-    for step in range(4):
-        st3 = torch.zeros(6, 4096, device = 'cuda', dtype = torch.int32); h3 = torch.zeros(4096, 2, device = 'cuda', dtype = torch.int32)
-        c3 = torch.tensor([0, step], device = 'cuda', dtype = torch.int32)
-        ops.sample_tokens(lg, 16, None, Vs, 10, st3, 4096, h3, 2, -1, som, 0, 10 ** 6, T, minp, 777, c3, 1)
-        counts += torch.bincount(st3[2].long(), minlength = Vs).float()[:Vs]
-    torch.cuda.synchronize()
-    x = base / T
-    p = x.softmax(-1)
-    keep = p >= minp * p.max()                                          # min-p over ALL logits (T.py:574-578) ...
-    keep[10:] = False                                                   # ... then the text-only restriction (T.py:2697): ids 10, 11 carry the largest logits
-    want_p = torch.where(keep, p, torch.zeros_like(p)); want_p = want_p / want_p.sum()
-    freq = counts / counts.sum()
-    assert (counts[~keep] == 0).all()
-    assert (freq - want_p).abs().max().item() < 0.02, (freq, want_p)
-    # decode_prep
-    st4 = torch.zeros(6, 4, device = 'cuda', dtype = torch.int32)
-    st4[0] = torch.tensor([3, 0, 99, 50]); st4[1] = torch.tensor([2, 0, 40, 7]); st4[2] = torch.tensor([11, 12, 13, 14])
-    meta = torch.zeros(8, 4, device = 'cuda', dtype = torch.int32); c4 = torch.zeros(2, device = 'cuda', dtype = torch.int32)
-    ops.decode_prep(st4, 4, 100, 2, meta[0], meta[1], meta[2], meta[3], meta[4], meta[5], meta[6], meta[7], c4)
-    torch.cuda.synchronize()
-    base_rows = torch.tensor([200, 300, 400, 500], device = 'cuda', dtype = torch.int32)
-    assert torch.equal(meta[0], st4[2]) and torch.equal(meta[1], st4[1]) and torch.equal(meta[2], base_rows + st4[0]) and torch.equal(meta[3], meta[2])
-    assert meta[4].tolist() == [0, 1, 2, 3] and meta[5].tolist() == [1, 2, 3, 4] and torch.equal(meta[6], base_rows) and torch.equal(meta[7], base_rows + st4[0] + 1)
-    assert c4.tolist() == [0, 1]
-
-
-def test_ode_kernels_follow_the_midpoint_rule(ops):
-    """tfx_ode_pre / tfx_ode_post over a table from decode.midpoint_table integrate dy/dt = a(t) y exactly like the host-side midpoint loop"""
-    from transfusion_pytorch_b200.decode import midpoint_table
-    steps, n = 6, 1000
-    tab = midpoint_table(steps, 'cuda')
-    y = torch.randn(n, device = 'cuda'); y0 = y.clone()
-    fprev = torch.zeros(n, device = 'cuda'); x = torch.zeros(2 * n, device = 'cuda'); ct = torch.zeros(3, device = 'cuda')
-    idx = torch.zeros(1, device = 'cuda', dtype = torch.int32)
-    f = lambda t, v: (0.5 - t) * v + 0.1
-    for e in range(2 * (steps - 1)):
-        ops.ode_pre(y, fprev, x, n, 2, tab, idx, ct, 3)
-        t = ct[0].item()
-        assert torch.equal(x[:n], x[n:]) and (ct == ct[0]).all()
-        pc, pu = f(t, x[:n]) * 1.5, f(t, x[:n]) * 0.5                   # cfg 2: u + 2 (c - u) = 2.5 f ... use cfg = 0.5: u + 0.5 (c - u) = f
-        ops.ode_post(y, fprev, pc, pu, 0.5, n, tab, idx)
-        ops.counter_inc(idx)
-    grid = torch.linspace(0, 1, steps)
-    w = y0.clone()
-    for t0, t1 in zip(grid[:-1], grid[1:]):
-        dt = (t1 - t0).item()
-        k1 = f(t0.item(), w)
-        w = w + dt * f(t0.item() + 0.5 * dt, w + 0.5 * dt * k1)
-    torch.cuda.synchronize()
-    assert torch.allclose(y, w, atol = 1e-5, rtol = 1e-5)
-
 def test_attn_residual_deferred_backward_chain_vs_autograd(ops):
     """tfx_attn_residual_bwd2: a stack of 4 AttentionResiduals over 5 hiddens (layer i mixes h_0..h_{i+1}), loss = sum_i <x_i, R_i>.  The deferred kernels
     assemble the COMPLETE gradient of each hidden once (own layer + stored scalars of the later layers) and must equal autograd's sum over layers."""

@@ -143,8 +143,9 @@ __global__ void __launch_bounds__(ROW_THREADS) sample_tokens_k(const float* __re
       const float x = lr[c] * it;
       if (x - mx < thr) continue;
       const unsigned long long h = mix64(seed ^ mix64((step << 40) ^ ((unsigned long long)s << 20) ^ (unsigned long long)c));
-      const float u = ((float)(h >> 40) + 0.5f) * (1.f / 16777216.f);         // (0, 1)
-      const float gmb = -__logf(-__logf(u));
+      // 23 bits: (k + 1/2) 2^-23 is exact in fp32 and lies in [2^-24, 1 - 2^-24].  (24 bits + 0.5 rounds 2^24 - 1/2 up to u = 1, a +inf Gumbel.)
+      const float u = ((float)(h >> 41) + 0.5f) * (1.f / 8388608.f);
+      const float gmb = -logf(-logf(u));                   // __logf's absolute error near u = 1 is as large as -log u itself
       const float y = x + gmb;
       if (y > best) { best = y; bi = c; }
     }
