@@ -66,6 +66,11 @@ int tfx_gemm_qkvg(const void* u, long long ldu, const void* W, long long ldw, in
                   const float* q_gamma, const float* k_gamma, const int* rope_pos, const float* rope_cs_t /* [32][rope_len][2], see tfx_rope_table */, int rope_len,
                   const int* kv_rows, float* mix_pre, void* stream);
 
+/* the same GEMM for `qk_rmsnorm = False` (T.py:949-951 skipped): q, k = RoPE(u W^T) with no norm, so no qk_inv and no gammas; v, gates,
+ * mix_pre and the kv_rows append are those of tfx_gemm_qkvg (same accumulators, bit for bit). */
+int tfx_gemm_qkvg_rope(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates,
+                       const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream);
+
 /* branch output projection + AdaptiveWrapper output gate + residual:
  *   y = [A | A2] W^T + bias ;  x_out = x_res + y * (cond_row[m] >= 0 ? zgate[cond_row[m]] : layerscale + 1)
  * to_out (T.py:1031) / FeedForward net.3 (T.py:849) with T.py:765-769 and the residual adds T.py:1238,1242;
@@ -114,6 +119,11 @@ int tfx_attn_bwd_tc(const void* q, const void* k, const void* v, const void* do_
 int tfx_qk_bwd_pack(const float* dq, const float* dk, const void* q_bf16, const void* k_bf16, const float* qk_inv, const float* q_gamma, const float* k_gamma,
                     const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16, long long out_ld,
                     float* dq_gamma, float* dk_gamma, int M, int H, void* stream);
+
+/* backward of the RoPE-only epilogue (tfx_gemm_qkvg_rope): d q_pre = R(pos)^T dq, d k_pre = R(pos)^T dk and the gate-logit column of
+ * tfx_qk_bwd_pack, packed into the same d[q | k | . | gates] layout */
+int tfx_qk_bwd_pack_rope(const float* dq, const float* dk, const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16,
+                         long long out_ld, int M, int H, void* stream);
 
 /* AttentionResidual backward with DEFERRED assembly (exact; rowops.cu): instead of read-modify-writing the gradient of every earlier hidden at every layer, layer i
  * stores three scalars per (token, hidden) and the complete gradient of ONE hidden is assembled when the backward pass needs it:

@@ -24,6 +24,7 @@ SIGNATURES = {
     'tfx_gemm_store_items': [I, I, I, I, I, I, VP],
     'tfx_gemm_store': [VP, LL, I, VP, LL, I, I, I, I, VP, LL, VP, LL, VP, VP, F, I, I, VP],
     'tfx_gemm_qkvg': [VP, LL, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP],
+    'tfx_gemm_qkvg_rope': [VP, LL, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, I, VP, VP, VP],
     'tfx_gemm_resid': [VP, LL, VP, LL, I, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, VP, LL, VP, VP],
     'tfx_gemm_geglu': [VP, LL, VP, LL, VP, I, I, I, VP, VP, VP],
     'tfx_gemm_geglu_drop': [VP, LL, VP, LL, VP, I, I, I, VP, VP, VP, F, I, VP],
@@ -34,6 +35,7 @@ SIGNATURES = {
     'tfx_attn_bwd': [VP, VP, VP, VP, LL, LL, LL, LL, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP, LL, I, I, F, F, VP, VP],
     'tfx_attn_bwd_tc': [VP, VP, VP, VP, LL, LL, LL, LL, VP, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP, LL, I, I, F, F, VP, VP],
     'tfx_qk_bwd_pack': [VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, LL, VP, VP, I, I, VP],
+    'tfx_qk_bwd_pack_rope': [VP, VP, VP, VP, VP, VP, VP, LL, I, I, VP],
     'tfx_adaln_fwd': [VP, VP, VP, LL, VP, VP, VP, I, I, VP],
     'tfx_adaln_bwd': [VP, VP, VP, VP, VP, LL, VP, VP, VP, LL, VP, I, I, VP],
     'tfx_resid_bwd': [VP, VP, VP, VP, LL, VP, VP, VP, LL, VP, VP, I, I, VP],

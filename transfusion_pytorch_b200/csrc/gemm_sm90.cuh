@@ -19,7 +19,7 @@
 //        the staging tiles.  GEGLU reads its whole accumulator row first and hands the tile on right then; its warpgroups stage
 //        through separate tiles, so the GELU math and stores of item j-1 overlap item j's accumulator write.
 // In the epilogue each thread of the warpgroup owns ONE accumulator row (warp q = 0..3: rows 32 q .. + 31, all 128 columns), the
-// layout the per-row epilogue math (qk-RMSNorm, RoPE, gate select) wants.
+// layout the per-row epilogue math (qk-RMSNorm, RoPE, gate select) wants.  EPI_QKVG_ROPE is EPI_QKVG without the qk-RMSNorm.
 //
 // Epilogue global traffic is staged through a per-warp 32 x 128 B shared-memory tile (XOR-swizzled 16 B chunks) so that every
 // global load / store instruction covers whole 64 / 128-byte row segments.  Apart from GEGLU, one warpgroup runs an epilogue at a
@@ -39,7 +39,8 @@ constexpr int GEMM_BN = 128;
 constexpr int GEMM_BK = 64;     // 64 bf16 = 128 B = one swizzle atom row
 constexpr int GEMM_UK = 16;     // wgmma K for 16-bit inputs
 
-enum : int { EPI_STORE = 0, EPI_QKVG = 1, EPI_RESID = 2, EPI_GEGLU = 3, EPI_GEGLU_DROP = 4 };   // GEGLU_DROP: GEGLU with FFN dropout on h
+// GEGLU_DROP: GEGLU with FFN dropout on h.  QKVG_ROPE: QKVG without the qk-RMSNorm (`qk_rmsnorm = False`): q, k = RoPE(acc), no qk_inv
+enum : int { EPI_STORE = 0, EPI_QKVG = 1, EPI_RESID = 2, EPI_GEGLU = 3, EPI_GEGLU_DROP = 4, EPI_QKVG_ROPE = 5 };
 
 struct GemmParams {
   int M, N, K;                 // D is M x N, reduction K
@@ -87,7 +88,7 @@ template <int EPI> struct GemmCfg {
   // per-warp staging: 32 rows x 128 B; RESID adds a 64-byte-pitch bf16 tile (2 KB).  Four warps (one epilogue warpgroup at a
   // time), except GEGLU: its warpgroups hand the accumulator tile over before their epilogues end, so each has its own four.
   static constexpr int STG_WARP = EPI == 2 ? 4096 + 2048 : 4096;
-  static constexpr int STAGING = (EPI >= 3 ? 8 : 4) * STG_WARP;
+  static constexpr int STAGING = (EPI == EPI_GEGLU || EPI == EPI_GEGLU_DROP ? 8 : 4) * STG_WARP;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ACC_BYTES + STAGING + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one block");
 };
@@ -498,7 +499,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int rows_valid = min(32, p.M - wrow0);            // may be <= 0
       const int col0 = n_blk * BN;
       int qk_pos = 0;
-      if constexpr (EPI == EPI_QKVG) { qk_pos = row_ok ? p.rope_pos[row] : 0; }
+      if constexpr (EPI == EPI_QKVG || EPI == EPI_QKVG_ROPE) { qk_pos = row_ok ? p.rope_pos[row] : 0; }
       if constexpr (EPI == EPI_RESID) { qk_pos = (row_ok && p.cond_row) ? p.cond_row[row] : -1; }      // (reused as the condition row)
 
       if constexpr (EPI == EPI_STORE) {
@@ -510,7 +511,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           acc_ld32(acc, erow, c * 32, r);
           store_slice(p, sw, lane, r, cbase, [&](int i) { return wrow0 + i; });
         }
-      } else if constexpr (EPI == EPI_QKVG) {
+      } else if constexpr (EPI == EPI_QKVG || EPI == EPI_QKVG_ROPE) {
         const int tps = p.H >> 1;             // tiles per section
         const int kind = n_blk / tps;         // 0 q, 1 k, 2 v, 3 gates
         const int tis = n_blk - kind * tps;   // tile in section
@@ -524,13 +525,16 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             uint32_t r0[32], r1[32];
             acc_ld32(acc, erow, hh * 64, r0);
             acc_ld32(acc, erow, hh * 64 + 32, r1);
-            float ss = 0.f;
+            float sc = 1.f;                               // qk-RMSNorm: 8 / |x| (times gamma + 1 per dim below)
+            if constexpr (EPI == EPI_QKVG) {
+              float ss = 0.f;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) { float a = __uint_as_float(r0[j]), b = __uint_as_float(r1[j]); ss += a * a + b * b; }
-            const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
+              for (int j = 0; j < 32; ++j) { float a = __uint_as_float(r0[j]), b = __uint_as_float(r1[j]); ss += a * a + b * b; }
+              const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
+              if (row_ok) p.qk_inv[(long long)row * 2 * p.H + kind * p.H + tis * 2 + hh] = inv;
+              sc = inv * 8.f;
+            }
             const int head = tis * 2 + hh;
-            if (row_ok) p.qk_inv[(long long)row * 2 * p.H + kind * p.H + head] = inv;
-            const float sc = inv * 8.f;
             uint32_t outw[32];
 #pragma unroll
             for (int dh = 0; dh < 2; ++dh) {              // the head's two 32-dim halves
@@ -538,9 +542,12 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
               for (int i = 0; i < 16; ++i) {
                 const int d0 = dh * 32 + 2 * i;
-                const float2 gm = *reinterpret_cast<const float2*>(gamma + d0);
-                const float y0 = __uint_as_float(rr[2 * i]) * sc * (gm.x + 1.f);
-                const float y1 = __uint_as_float(rr[2 * i + 1]) * sc * (gm.y + 1.f);
+                float y0 = __uint_as_float(rr[2 * i]), y1 = __uint_as_float(rr[2 * i + 1]);
+                if constexpr (EPI == EPI_QKVG) {
+                  const float2 gm = *reinterpret_cast<const float2*>(gamma + d0);
+                  y0 = y0 * sc * (gm.x + 1.f);
+                  y1 = y1 * sc * (gm.y + 1.f);
+                }
                 const float2 cc = cs[(long long)(dh * 16 + i) * p.rope_len];
                 outw[dh * 16 + i] = pack_bf16(y0 * cc.x - y1 * cc.y, y1 * cc.x + y0 * cc.y);
               }

@@ -819,6 +819,51 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_k(const float* __rest
   }
 }
 
+// ------------------------------------------------------------------------------------ RoPE backward (qk_rmsnorm = False), packs d[q|k|.|gates]
+// forward (GEMM epilogue EPI_QKVG_ROPE): q = R(pos) x.  d x = R(pos)^T d q per interleaved pair; no saved values are needed.  Same lane
+// layout as qk_bwd_pack_k: 8 lanes per head, a lane owns 8 consecutive dims (4 rope pairs), 4 heads per pass.
+__global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_rope_k(const float* __restrict__ dq, const float* __restrict__ dk, const int* __restrict__ rope_pos,
+                                                                 const float2* __restrict__ rope_cs, const float* __restrict__ gates, const float* __restrict__ dsum,
+                                                                 __nv_bfloat16* __restrict__ out, long long out_ld, int M, int H, int tpw) {
+  const int lane = threadIdx.x & 31;
+  const int sub = lane & 7, hq = lane >> 3;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);
+  const int HI = H * 64;
+  for (int row = r0; row < r1; ++row) {
+    float cs[8];   // (cos, sin) of the lane's 4 rope pairs
+    {
+      const float4* cp = reinterpret_cast<const float4*>(rope_cs + (long long)rope_pos[row] * 32 + sub * 4);
+      const float4 c0 = cp[0], c1 = cp[1];
+      cs[0] = c0.x; cs[1] = c0.y; cs[2] = c0.z; cs[3] = c0.w; cs[4] = c1.x; cs[5] = c1.y; cs[6] = c1.z; cs[7] = c1.w;
+    }
+    for (int h0 = 0; h0 < H; h0 += 4) {
+      const int h = h0 + hq;
+      if (h >= H) continue;
+      const long long off = (long long)row * HI + h * 64 + sub * 8;
+      const float4 da[2] = {*reinterpret_cast<const float4*>(dq + off), *reinterpret_cast<const float4*>(dk + off)};
+      const float4 db[2] = {*reinterpret_cast<const float4*>(dq + off + 4), *reinterpret_cast<const float4*>(dk + off + 4)};
+#pragma unroll
+      for (int which = 0; which < 2; ++which) {
+        const float dr[8] = {da[which].x, da[which].y, da[which].z, da[which].w, db[which].x, db[which].y, db[which].z, db[which].w};
+        uint32_t w[4];
+#pragma unroll
+        for (int pr = 0; pr < 4; ++pr) {
+          const float c = cs[2 * pr], sn = cs[2 * pr + 1];
+          w[pr] = pack2_bf16(dr[2 * pr] * c + dr[2 * pr + 1] * sn, dr[2 * pr + 1] * c - dr[2 * pr] * sn);     // un-rotate (R^T)
+        }
+        *reinterpret_cast<uint4*>(out + (long long)row * out_ld + which * HI + h * 64 + sub * 8) = make_uint4(w[0], w[1], w[2], w[3]);
+      }
+    }
+    // gate logits: d g = (1 - sigmoid(g)) * sum_d dO_gated * O_gated  (as in qk_bwd_pack_k)
+    if (lane < H) {
+      const float gl = gates[(long long)row * H + lane];
+      const float sg = 1.f / (1.f + __expf(-gl));
+      out[(long long)row * out_ld + 3 * HI + lane] = __float2bfloat16((1.f - sg) * dsum[(long long)row * H + lane]);
+    }
+  }
+}
+
 int num_sms();
 static inline int row_grid(int M, int sms) {
   long long blocks = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
@@ -1012,6 +1057,15 @@ int tfx_qk_bwd_pack(const float* dq, const float* dk, const void* q_bf16, const 
   qk_bwd_pack_k<<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, (const __nv_bfloat16*)q_bf16, (const __nv_bfloat16*)k_bf16, qk_inv, q_gamma, k_gamma, rope_pos,
                                                                      (const float2*)rope_cs, gates, dsum, (__nv_bfloat16*)dqkvg_bf16, out_ld, dq_gamma, dk_gamma, M, H, tpw);
   return check_launch("qk_bwd_pack");
+}
+
+int tfx_qk_bwd_pack_rope(const float* dq, const float* dk, const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16,
+                         long long out_ld, int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(H >= 1 && H <= 32, "qk_bwd_pack_rope: heads %d out of range", H);
+  const int tpw = 8;
+  qk_bwd_pack_rope_k<<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, rope_pos, (const float2*)rope_cs, gates, dsum_mh, (__nv_bfloat16*)dqkvg_bf16, out_ld, M, H, tpw);
+  return check_launch("qk_bwd_pack_rope");
 }
 
 }  // extern "C"

@@ -159,6 +159,10 @@ class Engine:
         self.W = 2 * self.depth                     # AdaptiveWrappers
         self.softcap = tr.softcap_value
         self.laser, self.laser_clamp, self.vres = tr.attn_laser, tr.laser_softclamp_value, tr.use_value_residual
+        # qk_rmsnorm = False (T.py:949-951 skipped): q, k are RoPE(u W^T) only, so no bound on the logits follows from the gammas and every layer runs
+        # the general (running-maximum) attention kernels; the q / k norm gammas stay out of the flat buffers (their .grad stays None, as in the reference)
+        self.qk_norm = bool(getattr(tr, 'qk_rmsnorm', True))
+        self.fastp = None                           # per layer: bounded-logit attention parameters (tfx_attn_fast_params), qk_rmsnorm models only
         self.clean, self.clean_eps = bool(getattr(model, 'model_output_clean', False)), float(getattr(model, 'eps', 1e-2))
         self.posemb = tuple(bool(a) for a in getattr(model, 'add_pos_emb', ()))      # per modality type: axial positional embedding on the latent tokens
         self.scale = 64 ** -0.5
@@ -182,6 +186,8 @@ class Engine:
         for mod in list(m.modality_encoder) + list(m.modality_decoder):
             if mod is not None:
                 skip |= {id(p) for p in mod.parameters()}
+        if not self.qk_norm:                        # built but unused without the qk-RMSNorm (T.py:886-888, 949-951): no gradient, no optimizer state
+            skip |= {id(p) for n, p in m.named_parameters() if n.endswith(('.fn.q_norm.gamma', '.fn.k_norm.gamma'))}
         return [(n, p) for n, p in m.named_parameters() if p.requires_grad and id(p) not in skip]
 
     def attach(self):
@@ -353,11 +359,12 @@ class Engine:
             self._build_pack_jobs()
         self.ops.cast_pack_multi(self._pack_tab, self._pack_blk_job, self._pack_blk_first, self._pack_nblocks)
         # per layer: is the bounded-logit (wgmma) attention path valid for the current q/k norm gammas?  (device-side decision)
-        if getattr(self, 'fastp', None) is None or self.fastp.device != self.device:
-            self.fastp = torch.zeros(self.depth, 8, device = self.device, dtype = F32)
-        for i in range(self.depth):
-            pre = f'transformer.layers.{i}.1.fn'
-            self.ops.attn_fast_params(self.P(f'{pre}.q_norm.gamma'), self.P(f'{pre}.k_norm.gamma'), 64, self.scale, self.softcap, self.fastp[i])
+        if self.qk_norm:
+            if self.fastp is None or self.fastp.device != self.device:
+                self.fastp = torch.zeros(self.depth, 8, device = self.device, dtype = F32)
+            for i in range(self.depth):
+                pre = f'transformer.layers.{i}.1.fn'
+                self.ops.attn_fast_params(self.P(f'{pre}.q_norm.gamma'), self.P(f'{pre}.k_norm.gamma'), 64, self.scale, self.softcap, self.fastp[i])
         self._dirty = False
 
     # ------------------------------------------------------------------ descriptor upload
@@ -547,11 +554,17 @@ class Engine:
             else:
                 # inference shares one buffer set across layers, but the value residual reads the FIRST layer's values in every later layer
                 k = self.buf(f'{lt}k', (M, HI), BF16); v = self.buf(f'{lt}v0' if (self.vres and i == 0) else f'{lt}v', (M, HI), BF16)
-            gates = self.buf(f'{lt}g', (M, H), F32); qk_inv = self.buf(f'{lt}qi', (M, 2 * H), F32)
+            gates = self.buf(f'{lt}g', (M, H), F32)
             has_mix = self.vres and i > 0
             mixpre = self.buf(f'{lt}mix', (M, H), F32) if has_mix else None
-            o.gemm_qkvg(uA, D, pk[f'qkvg{i}'], D, M, H, D, q, k, v, gates, qk_inv, self.P(f'{pre}.1.fn.q_norm.gamma'), self.P(f'{pre}.1.fn.k_norm.gamma'),
-                        dv['rope_pos'], self.ws['rope_cs_t'], int(self.ws['rope_cs_t'].shape[1]), kv_rows, mixpre)
+            if self.qk_norm:
+                qk_inv = self.buf(f'{lt}qi', (M, 2 * H), F32)
+                o.gemm_qkvg(uA, D, pk[f'qkvg{i}'], D, M, H, D, q, k, v, gates, qk_inv, self.P(f'{pre}.1.fn.q_norm.gamma'), self.P(f'{pre}.1.fn.k_norm.gamma'),
+                            dv['rope_pos'], self.ws['rope_cs_t'], int(self.ws['rope_cs_t'].shape[1]), kv_rows, mixpre)
+            else:
+                qk_inv = None
+                o.gemm_qkvg_rope(uA, D, pk[f'qkvg{i}'], D, M, H, D, q, k, v, gates, dv['rope_pos'], self.ws['rope_cs_t'], int(self.ws['rope_cs_t'].shape[1]),
+                                 kv_rows, mixpre)
             if has_mix:                                  # learned value residual (T.py:956-960): v = v mix + v_first_layer (1 - mix), in place (also on the cache rows)
                 v_first = cache.v[0] if cache is not None else st['layers'][0]['v']
                 o.vmix_fwd(v, HI, kv_rows, v_first, HI, mixpre, self.P(f'{pre}.1.fn.to_learned_value_residual.0.bias'), M, H)
@@ -562,14 +575,16 @@ class Engine:
                 att_gates = None
             att = self.buf(f'{lt}o', (M, HI), BF16); lse = self.buf(f'{lt}lse', (H, M), F32)
             o_l = self.buf(f'{lt}ol', (M, HI), BF16) if self.laser else att
-            fp = self.fastp[i]
+            fp = self.fastp[i] if self.qk_norm else None
             if getattr(rb, 'single_row_tiles', False):
                 # text decode: one query row per sample against its cache slab (split-KV decode kernel)
                 o.attn_decode(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['tile_q0'], dv['tile_kv0'], dv['tile_kvend'], n_tiles, o_l, HI, self.scale, self.softcap)
             else:
-                # both kernels are enqueued; the one whose precondition (read from `fp` on the device) fails returns immediately
-                o.attn_fwd_tc(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['t2_q0'], dv['t2_qend'], dv['t2_kv0'], dv['t2_kvend'], int(rb.t2_q0.shape[0]),
-                              o_l, HI, lse, M, M_kv, self.scale, self.softcap, fp)
+                # both kernels are enqueued; the one whose precondition (read from `fp` on the device) fails returns immediately.  Without the
+                # qk-RMSNorm only the general kernel runs (fp = None)
+                if self.qk_norm:
+                    o.attn_fwd_tc(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['t2_q0'], dv['t2_qend'], dv['t2_kv0'], dv['t2_kvend'], int(rb.t2_q0.shape[0]),
+                                  o_l, HI, lse, M, M_kv, self.scale, self.softcap, fp)
                 o.attn_fwd(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['tile_q0'], dv['tile_qend'], dv['tile_kv0'], dv['tile_kvend'], n_tiles,
                            o_l, HI, lse, M, self.scale, self.softcap, fp)
             if self.laser:
@@ -892,9 +907,10 @@ class Engine:
             dqkvg = self.buf('dqkvg', (M, self.NQ), BF16)
             if i == self.depth - 1:
                 dqkvg[:, 3 * HI + H:].zero_()   # pad columns are never written by the kernels; cleared once per backward (inside captured graphs too)
-            fp = self.fastp[i]
-            o.attn_bwd_tc(L['q'], L['k'], L['v_att'], dop, HI, HI, HI, HI, L['lse'], dsum_hm, dv['kv_limit'], dv['k2_kv0'], dv['k2_kvend'], dv['k2_q0'], dv['k2_qend'],
-                          dv['k2_order'], int(rb.k2_kv0.shape[0]), dq, dk, dqkvg[:, 2 * HI:], self.NQ, M, H, self.scale, self.softcap, fp)
+            fp = self.fastp[i] if self.qk_norm else None
+            if self.qk_norm:
+                o.attn_bwd_tc(L['q'], L['k'], L['v_att'], dop, HI, HI, HI, HI, L['lse'], dsum_hm, dv['kv_limit'], dv['k2_kv0'], dv['k2_kvend'], dv['k2_q0'], dv['k2_qend'],
+                              dv['k2_order'], int(rb.k2_kv0.shape[0]), dq, dk, dqkvg[:, 2 * HI:], self.NQ, M, H, self.scale, self.softcap, fp)
             o.attn_bwd(L['q'], L['k'], L['v_att'], dop, HI, HI, HI, HI, L['lse'], dsum_hm, dv['kv_limit'], dv['kt_kv0'], dv['kt_kvend'], dv['kt_q0'], dv['kt_qend'],
                        int(rb.kt_kv0.shape[0]), dq, dk, dqkvg[:, 2 * HI:], self.NQ, M, H, self.scale, self.softcap, fp)
             dv_cols = dqkvg[:, 2 * HI:]
@@ -911,8 +927,11 @@ class Engine:
                 else:
                     dqkvg[:, 3 * HI + H:3 * HI + 2 * H].zero_()      # the first layer has no mix Linear: its column block must not carry layer 1's values
                     o.add_f32_into_bf16(dv_cols, self.NQ, dv0, HI, M, HI)
-            o.qk_bwd_pack(dq, dk, L['q'], L['k'], L['qk_inv'], self.P(f'{pre}.1.fn.q_norm.gamma'), self.P(f'{pre}.1.fn.k_norm.gamma'), dv['rope_pos'],
-                          self.ws['rope_cs'], L['gates'], dsum_mh, dqkvg, self.NQ, self.G(f'{pre}.1.fn.q_norm.gamma'), self.G(f'{pre}.1.fn.k_norm.gamma'), M, H)
+            if self.qk_norm:
+                o.qk_bwd_pack(dq, dk, L['q'], L['k'], L['qk_inv'], self.P(f'{pre}.1.fn.q_norm.gamma'), self.P(f'{pre}.1.fn.k_norm.gamma'), dv['rope_pos'],
+                              self.ws['rope_cs'], L['gates'], dsum_mh, dqkvg, self.NQ, self.G(f'{pre}.1.fn.q_norm.gamma'), self.G(f'{pre}.1.fn.k_norm.gamma'), M, H)
+            else:
+                o.qk_bwd_pack_rope(dq, dk, dv['rope_pos'], self.ws['rope_cs'], L['gates'], dsum_mh, dqkvg, self.NQ, M, H)
             o.gemm_store(dqkvg, self.NQ, 0, pk[f'qkvg{i}'], D, 1, M, D, self.NQ, du, D, None, 0, None, None, 1.0, 0, 1)
             o.gemm_store(dqkvg, self.NQ, 1, L['uA'], D, 1, self.NQ, D, M, self.gflat, 0, None, 0, None, lm['qkvg_rows'], 1.0, 1, ksplit(self.NQ, D))
             o.adaln_bwd(du, L['x_a'], L['statsA'], cond_row, st['tab'][:, wA * 3 * D:] if nc > 0 else None, tab_ld, self.P(f'{pre}.1.layernorm_gamma'), gx,

@@ -8,7 +8,8 @@ the block stack, attention, loss heads and optimizer runs in the sm_90a kernels 
 driven by `engine.Engine` over the ragged descriptor of `modality_processing.pack_batch`.
 
 Out of scope here (raise loudly): U-Net pre/post encoders (`pre_post_transformer_enc_dec`), attention dropout, dim_head != 64, a custom
-`loss_fn` of `SelfMaskedRepTraining`.
+`loss_fn` of `SelfMaskedRepTraining`.  `qk_rmsnorm = False` is supported: the q / k norm gammas are still built (same state-dict keys) and get
+no gradient, as in the reference.
 """
 from __future__ import annotations
 
@@ -222,7 +223,6 @@ class Transformer(Module):
         # branch on CUDA (T.py:987-995), which applies no attention dropout, so there `dropout` is accepted and has no effect.
         if dropout != 0. and not use_flex_attn: unsupported.append('dropout > 0 (attention dropout) without use_flex_attn')
         if use_value_residual and heads > 16: unsupported.append('use_value_residual with heads > 16')
-        if not qk_rmsnorm: unsupported.append('qk_rmsnorm = False')
         extra = set(attn_kwargs) - {'softcap_value', 'laser_softclamp_value'}
         if extra: unsupported.append(f'attn_kwargs {sorted(extra)}')
         extra = set(ff_kwargs) - {'dropout'}         # FeedForward(dim, mult, dropout) (T.py:837-850): dropout is its only option besides the two above
@@ -233,6 +233,7 @@ class Transformer(Module):
         self.use_flex_attn = use_flex_attn           # accepted: the fused kernel IS the span-aware attention
         self.use_value_residual = bool(use_value_residual)
         self.attn_laser = bool(attn_laser)
+        self.qk_rmsnorm = bool(qk_rmsnorm)           # False: q, k = RoPE(to_qk(x)) without the norms (T.py:949-951); their gammas stay built (T.py:886-888)
         self.laser_softclamp_value = float(attn_kwargs.get('laser_softclamp_value', 15.))
         self.softcap_value = float(attn_kwargs.get('softcap_value', 50.))
         self.ff_inner = int(dim * ff_expansion_factor * 2 / 3)
