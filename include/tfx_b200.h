@@ -127,7 +127,8 @@ int tfx_qk_bwd_pack_rope(const float* dq, const float* dk, const int* rope_pos, 
 
 /* AttentionResidual backward with DEFERRED assembly (exact; rowops.cu): instead of read-modify-writing the gradient of every earlier hidden at every layer, layer i
  * stores three scalars per (token, hidden) and the complete gradient of ONE hidden is assembled when the backward pass needs it:
- *   G_k = sum_{i' >= k-1} [a_{i',k} dx_{i'} + c1_{i',k} w_{i'}] - (sum c2_{i',k}) h_k.
+ *   G_k = sum_{i' >= k-1} [a_{i',k} dx_{i'} + c1_{i',k} w_{i'}] - (sum c2_{i',k}) h_k,
+ * with c2 = 0 on a row shorter than the 1e-12 norm clamp (the clamped norm is a constant for the gradient, as in F.normalize).
  * own = 1: layer with hiddens h_0..h_{n-1}; writes the scalars of h_0..h_{n-2} to scalars_out[token][k][3] (row stride scalar_stride floats), the parameter gradients,
  * and grad_hidden = G_{n-1} from its own term plus the n_later later layers (dx_later[j], scalars_later[j] -> element [token 0][k = n-1][0], gammas / pseudo_queries[1 + j]).
  * own = 0: assembly only (gammas[0] / pseudo_queries[0] unused): the gradient of h_0 after the first layer.

@@ -311,6 +311,7 @@ __global__ void __launch_bounds__(ROW_THREADS) attn_res_fwd_k(HiddenList hid, in
 // Layer i' adds to the gradient of every hidden k it mixes  a_k dx + c1_k w - c2_k h_k,  and to dw (-> d gamma, d pq)  c1_k h_k, where
 //     a_k = exp(sim_k - lse)  (the log-sum-exp saved by the forward),   ds_k = a_k (<h_k, dx> - <x_out, dx>),   c1_k = ds_k / |h_k|,   c2_k = ds_k <h_k, w> / |h_k|^3
 // (the softmax-backward mean  sum_k a_k <h_k, dx>  equals <x_out, dx>, x_out being the saved forward output, so every h_k is read once per layer).
+// |h_k| stands for max(|h_k|, 1e-12) as F.normalize clamps it; below the clamp the norm is a constant for the gradient, so c2_k = 0 there.
 // Adding these terms into dH_k at every layer would read-modify-write (i + 2) fp32 rows per token and layer.  Each term is (per-token scalars) x (a vector
 // that already exists: the incoming gradient dx_i', the layer's w_i', the hidden itself), so this kernel stores the three scalars per (token, layer, hidden) -
 // 12 bytes instead of 2 KB - and assembles the COMPLETE gradient of one hidden, once, when the backward pass needs it:
@@ -447,7 +448,7 @@ __global__ void __launch_bounds__(ROW_THREADS, 2) attn_res_bwd2_k(ResBwd2Args A,
         const float nrm = fmaxf(sqrtf(ss), 1e-12f), rn = 1.f / nrm;
         const float a = __expf(dot * rn - lse_r);
         const float ds = a * (da - mean_da);
-        const float c1 = ds * rn, c2 = ds * dot * rn * rn * rn;
+        const float c1 = ds * rn, c2 = sqrtf(ss) < 1e-12f ? 0.f : ds * dot * rn * rn * rn;   // clamped norm: a constant for the gradient
 #pragma unroll
         for (int i = 0; i < NCH * 4; ++i) accw[i] += c1 * h[i];
         if (k + 1 < A.L1) {
