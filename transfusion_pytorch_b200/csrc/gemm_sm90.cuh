@@ -79,6 +79,7 @@ struct GemmParams {
 };
 
 template <int EPI> struct GemmCfg {
+  static constexpr int BM = GEMM_BM;
   static constexpr int THREADS = 384;
   static constexpr int STAGES = 4;
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
@@ -329,6 +330,120 @@ __device__ __forceinline__ void store_slice(const GemmParams& p, uint8_t* sw, in
   }
 }
 
+// ------------------------------------------------------------------------------------------------ pipeline of both kernels
+// Persistent schedule: work items run over (k split, m unit, n tile), n fastest; an m unit is CL vertically adjacent BM-row tiles, one per
+// CTA of the cluster.
+template <int BM, int CL>
+struct GemmSched {
+  struct Work { int m_blk, n_blk, kb0, kb1; };
+  int n_tiles, unit_items, kb_total, kb_per_split, num_items;
+  __device__ __forceinline__ explicit GemmSched(const GemmParams& p) {
+    const int m_tiles = (p.M + BM - 1) / BM;
+    n_tiles = (p.N + GEMM_BN - 1) / GEMM_BN;
+    kb_total = (p.K + GEMM_BK - 1) / GEMM_BK;
+    kb_per_split = (kb_total + p.k_splits - 1) / p.k_splits;
+    unit_items = (m_tiles + CL - 1) / CL * n_tiles;
+    num_items = unit_items * p.k_splits;
+  }
+  // the tile of work item `item` that CTA `cta_rank` computes, and its k-blocks [kb0, kb1).  With CL = 2 and an odd tile count the last
+  // unit's second tile is past the end: TMA zero-fills it and every store is row-guarded.
+  __device__ __forceinline__ Work work(int item, int cta_rank) const {
+    const int split = item / unit_items;
+    const int rem = item - split * unit_items;
+    const int m_unit = rem / n_tiles;
+    const int kb0 = split * kb_per_split;
+    return {m_unit * CL + cta_rank, rem - m_unit * n_tiles, kb0, min(kb0 + kb_per_split, kb_total)};
+  }
+};
+
+// a slot of the STAGES-deep shared-memory ring and the parity of its current fill
+template <int STAGES>
+struct GemmRing {
+  int stage = 0; uint32_t phase = 0;
+  __device__ __forceinline__ void step() { if (++stage == STAGES) { stage = 0; phase ^= 1; } }
+};
+
+// Producer: once the ring slot is free, load k-block kb of the Cfg::BM-row A tile m_blk and the 128-row B tile n_blk into it, and step on.
+// TWO_A: a K-major A is the concatenation [A | A2] along K, with A2 (tmA2) from k = p.K1.  CL = 2: this CTA's half of the B tile (64 rows,
+// or one 64-wide MN block) goes to the same offset of both CTAs' rings.
+template <class Cfg, bool A_MN, bool B_MN, int CL, bool TWO_A>
+__device__ __forceinline__ void gemm_fill(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, GemmRing<Cfg::STAGES>& ring,
+                                          const CUtensorMap* tmA, const CUtensorMap* tmA2, const CUtensorMap* tmB, const GemmParams& p,
+                                          int kb, int m_blk, int n_blk, int cta_rank) {
+  constexpr int BM = Cfg::BM, BN = GEMM_BN;
+  mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1);
+  uint8_t* sA = smem + ring.stage * Cfg::STAGE_BYTES;
+  uint8_t* sB = sA + Cfg::A_BYTES;
+  uint64_t* bar = &full_bar[ring.stage];
+  mbar_expect_tx(bar, Cfg::STAGE_BYTES);
+  if (!A_MN) {
+    if (!TWO_A || kb * GEMM_BK < p.K1) tma_load_2d(tmA, bar, sA, kb * GEMM_BK, m_blk * BM);     // one 64 x BM box
+    else tma_load_2d(tmA2, bar, sA, kb * GEMM_BK - p.K1, m_blk * BM);
+  } else {
+#pragma unroll
+    for (int a = 0; a < BM / 64; ++a)
+      tma_load_2d(tmA, bar, sA + a * (GEMM_BK * 128), m_blk * BM + a * 64, kb * GEMM_BK);
+  }
+  if constexpr (CL > 1) {
+    if (!B_MN) tma_load_2d_multicast(tmB, bar, sB + cta_rank * (64 * 128), kb * GEMM_BK, n_blk * BN + cta_rank * 64, (uint16_t)3);
+    else tma_load_2d_multicast(tmB, bar, sB + cta_rank * (GEMM_BK * 128), n_blk * BN + cta_rank * 64, kb * GEMM_BK, (uint16_t)3);
+  } else if (!B_MN) {
+    tma_load_2d(tmB, bar, sB, kb * GEMM_BK, n_blk * BN);
+  } else {
+#pragma unroll
+    for (int a = 0; a < BN / 64; ++a)
+      tma_load_2d(tmB, bar, sB + a * (GEMM_BK * 128), n_blk * BN + a * 64, kb * GEMM_BK);
+  }
+  ring.step();
+}
+
+// Consumer main loop of one work item: k-blocks [kb0, kb1) into the accumulators of 128 tile rows (d0: rows 0-63, d1: rows 64-127), whose
+// A rows start a_off bytes into the slot's A tile.  Two wgmma.m64n128k16 per 16-deep k step.  A slot is released one k-block behind, once
+// wgmma.wait_group 1 shows its MMAs retired; the slot of the last k-block (-1 if none) is returned for gemm_drain.
+template <class Cfg, bool A_MN, bool B_MN, class Release>
+__device__ __forceinline__ int gemm_mainloop(uint8_t* smem, uint64_t* full_bar, GemmRing<Cfg::STAGES>& ring, uint32_t a_off, int kb0, int kb1,
+                                             float (&d0)[64], float (&d1)[64], Release& release) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+  int prev_stage = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&full_bar[ring.stage], ring.phase);
+    const uint32_t sA = smem_u32(smem + ring.stage * Cfg::STAGE_BYTES) + a_off;
+    const uint32_t sB = smem_u32(smem + ring.stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+    wgmma_reg_fence(d0);
+    wgmma_reg_fence(d1);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < GEMM_BK / GEMM_UK; ++k) {
+      const uint64_t db = B_MN ? wgmma_desc_sw128(sB + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
+                               : wgmma_desc_sw128(sB + k * (GEMM_UK * 2), 16, 1024);
+      // A rows 64-127: the second 64-wide MN block (MN-major) or 64 rows further down (K-major)
+      const uint64_t da0 = A_MN ? wgmma_desc_sw128(sA + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
+                                : wgmma_desc_sw128(sA + k * (GEMM_UK * 2), 16, 1024);
+      const uint64_t da1 = A_MN ? wgmma_desc_sw128(sA + GEMM_BK * 128 + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
+                                : wgmma_desc_sw128(sA + 64 * 128 + k * (GEMM_UK * 2), 16, 1024);
+      const uint32_t acc_flag = (kb > kb0 || k > 0) ? 1u : 0u;
+      wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d0, da0, db, acc_flag);
+      wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d1, da1, db, acc_flag);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();                        // the previous k-block's MMAs have retired: its smem slot is free
+    if (prev_stage >= 0) release(prev_stage);
+    prev_stage = ring.stage;
+    ring.step();
+  }
+  return prev_stage;
+}
+
+// after the main loop: every MMA retired, the accumulators fenced, the last slot released
+template <class Release>
+__device__ __forceinline__ void gemm_drain(float (&d0)[64], float (&d1)[64], int last_stage, Release& release) {
+  wgmma_wait<0>();
+  wgmma_reg_fence(d0);
+  wgmma_reg_fence(d1);
+  if (last_stage >= 0) release(last_stage);
+}
+
 template <bool A_MN, bool B_MN, int EPI, int CL>
 __global__ void __launch_bounds__(384, 1)
 gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
@@ -348,13 +463,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* empty_bar = bars + STAGES;        // [STAGES]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = (p.M + GEMM_BM - 1) / GEMM_BM;
-  const int n_tiles = (p.N + BN - 1) / BN;
-  const int kb_total = (p.K + GEMM_BK - 1) / GEMM_BK;
-  const int kb_per_split = (kb_total + p.k_splits - 1) / p.k_splits;
-  const int m_units = (m_tiles + CL - 1) / CL;            // a work item = CL vertically adjacent tiles, one per CTA of the cluster
-  const int unit_items = m_units * n_tiles;
-  const int num_items = unit_items * p.k_splits;
+  const GemmSched<GEMM_BM, CL> sched(p);
+  const int num_items = sched.num_items;
   const int cta_rank = CL > 1 ? (int)cluster_ctarank() : 0;
   const int first_item = blockIdx.x / CL, item_stride = gridDim.x / CL;
 
@@ -372,39 +482,11 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // ===================================================== TMA producer
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
-      int stage = 0; uint32_t phase = 0;
+      GemmRing<STAGES> ring;
       for (int item = first_item; item < num_items; item += item_stride) {
-        const int split = item / unit_items;
-        const int rem = item - split * unit_items;
-        const int m_unit = rem / n_tiles, n_blk = rem - m_unit * n_tiles;
-        const int m_blk = m_unit * CL + cta_rank;             // (past the last tile for an odd tile count: zero-filled by TMA, results discarded)
-        const int kb0 = split * kb_per_split;
-        const int kb1 = min(kb0 + kb_per_split, kb_total);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sB = sA + Cfg::A_BYTES;
-          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          if (!A_MN) {
-            if (kb * GEMM_BK < p.K1) tma_load_2d(&tmA, &full_bar[stage], sA, kb * GEMM_BK, m_blk * GEMM_BM);
-            else tma_load_2d(&tmA2, &full_bar[stage], sA, kb * GEMM_BK - p.K1, m_blk * GEMM_BM);
-          } else {
-#pragma unroll
-            for (int a = 0; a < GEMM_BM / 64; ++a)
-              tma_load_2d(&tmA, &full_bar[stage], sA + a * (GEMM_BK * 128), m_blk * GEMM_BM + a * 64, kb * GEMM_BK);
-          }
-          if constexpr (CL > 1) {        // this CTA's half of the B tile (64 rows, or one 64-wide MN block) into both CTAs
-            if (!B_MN) tma_load_2d_multicast(&tmB, &full_bar[stage], sB + cta_rank * (64 * 128), kb * GEMM_BK, n_blk * BN + cta_rank * 64, (uint16_t)3);
-            else tma_load_2d_multicast(&tmB, &full_bar[stage], sB + cta_rank * (GEMM_BK * 128), n_blk * BN + cta_rank * 64, kb * GEMM_BK, (uint16_t)3);
-          } else if (!B_MN) {
-            tma_load_2d(&tmB, &full_bar[stage], sB, kb * GEMM_BK, n_blk * BN);
-          } else {
-#pragma unroll
-            for (int a = 0; a < BN / 64; ++a)
-              tma_load_2d(&tmB, &full_bar[stage], sB + a * (GEMM_BK * 128), n_blk * BN + a * 64, kb * GEMM_BK);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
+        const auto w = sched.work(item, cta_rank);
+        for (int kb = w.kb0; kb < w.kb1; ++kb)
+          gemm_fill<Cfg, A_MN, B_MN, CL, true>(smem, full_bar, empty_bar, ring, &tmA, &tmA2, &tmB, p, kb, w.m_blk, w.n_blk, cta_rank);
       }
     }
   } else {
@@ -416,7 +498,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int quad = warp & 3;                 // epilogue rows 32 quad .. + 31; fragment rows 16 quad .. of each 64-row half
     uint8_t* sw = staging + ((GEGLU ? 4 * cw : 0) + quad) * Cfg::STG_WARP;
     const int erow = quad * 32 + lane;         // this thread's accumulator row in the epilogue
-    int stage = 0; uint32_t phase = 0;
+    GemmRing<STAGES> ring;
     // a consumed ring slot is released in every CTA that wrote into it
     auto release = [&](int s) {
       __syncwarp();
@@ -427,56 +509,20 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     };
     int nth = 0;                               // position of `item` in this CTA's sequence
     for (int item = first_item; item < num_items; item += item_stride, ++nth) {
-      const int split = item / unit_items;
-      const int rem = item - split * unit_items;
-      const int m_unit = rem / n_tiles, n_blk = rem - m_unit * n_tiles;
-      const int m_blk = m_unit * CL + cta_rank;               // a tile past the end has rows_valid <= 0: every store below is row-guarded
-      const int kb0 = split * kb_per_split;
-      const int kb1 = min(kb0 + kb_per_split, kb_total);
+      const auto [m_blk, n_blk, kb0, kb1] = sched.work(item, cta_rank);
       if ((nth & 1) != cw) {                                 // the other warpgroup's item: step over its k-blocks in the ring
-        const int s = stage + (kb1 - kb0);
-        stage = s % STAGES;
-        phase ^= (uint32_t)(s / STAGES) & 1u;
+        const int s = ring.stage + (kb1 - kb0);
+        ring.stage = s % STAGES;
+        ring.phase ^= (uint32_t)(s / STAGES) & 1u;
         continue;
       }
       // hand-offs pair up exactly: item nth waits for nth - 1's signal iff nth > 0, and signals iff there is an item nth + 1
       const bool has_next = item + item_stride < num_items;
       if (nth > 0) named_bar_sync(BAR_MMA + cw, 256);
       float d0[64], d1[64];                                   // accumulator rows 0-63 / 64-127
-#pragma unroll
-      for (int i = 0; i < 64; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
-      int prev_stage = -1;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-        const uint32_t sB = sA + Cfg::A_BYTES;
-        wgmma_reg_fence(d0);
-        wgmma_reg_fence(d1);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BK / GEMM_UK; ++k) {
-          const uint64_t db = B_MN ? wgmma_desc_sw128(sB + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
-                                   : wgmma_desc_sw128(sB + k * (GEMM_UK * 2), 16, 1024);
-          // A rows 64-127: the second 64-wide MN block (MN-major) or 64 rows further down (K-major)
-          const uint64_t da0 = A_MN ? wgmma_desc_sw128(sA + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
-                                    : wgmma_desc_sw128(sA + k * (GEMM_UK * 2), 16, 1024);
-          const uint64_t da1 = A_MN ? wgmma_desc_sw128(sA + GEMM_BK * 128 + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
-                                    : wgmma_desc_sw128(sA + 64 * 128 + k * (GEMM_UK * 2), 16, 1024);
-          const uint32_t acc_flag = (kb > kb0 || k > 0) ? 1u : 0u;
-          wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d0, da0, db, acc_flag);
-          wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d1, da1, db, acc_flag);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                        // the previous k-block's MMAs have retired: its smem slot is free
-        if (prev_stage >= 0) release(prev_stage);
-        prev_stage = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
+      const int last_stage = gemm_mainloop<Cfg, A_MN, B_MN>(smem, full_bar, ring, 0, kb0, kb1, d0, d1, release);
       if (has_next) named_bar_arrive(BAR_MMA + (cw ^ 1), 256);     // every k-block of this item is issued: the other main loop may start
-      wgmma_wait<0>();
-      wgmma_reg_fence(d0);
-      wgmma_reg_fence(d1);
-      if (prev_stage >= 0) release(prev_stage);
+      gemm_drain(d0, d1, last_stage, release);
 
       // ---- accumulator fragments -> shared fp32 tile, once the previous item's epilogue has finished reading it
       if (nth > 0) named_bar_sync(BAR_ACC + cw, 256);
@@ -756,12 +802,8 @@ gemm_sm90_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   uint64_t* empty_bar = full_bar + STAGES;                                     // [STAGES]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = (p.M + BM - 1) / BM;
-  const int n_tiles = (p.N + BN - 1) / BN;
-  const int kb_total = (p.K + GEMM_BK - 1) / GEMM_BK;
-  const int kb_per_split = (kb_total + p.k_splits - 1) / p.k_splits;
-  const int tiles = m_tiles * n_tiles;
-  const int num_items = tiles * p.k_splits;
+  const GemmSched<BM, 1> sched(p);
+  const int num_items = sched.num_items;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
@@ -775,34 +817,11 @@ gemm_sm90_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     // ===================================================== TMA producer
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
-      int stage = 0; uint32_t phase = 0;
+      GemmRing<STAGES> ring;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        const int split = item / tiles;
-        const int rem = item - split * tiles;
-        const int m_blk = rem / n_tiles, n_blk = rem - m_blk * n_tiles;
-        const int kb0 = split * kb_per_split;
-        const int kb1 = min(kb0 + kb_per_split, kb_total);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sB = sA + Cfg::A_BYTES;
-          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          if (!A_MN) {
-            tma_load_2d(&tmA, &full_bar[stage], sA, kb * GEMM_BK, m_blk * BM);           // one 64 x 256 box
-          } else {
-#pragma unroll
-            for (int a = 0; a < BM / 64; ++a)
-              tma_load_2d(&tmA, &full_bar[stage], sA + a * (GEMM_BK * 128), m_blk * BM + a * 64, kb * GEMM_BK);
-          }
-          if (!B_MN) {
-            tma_load_2d(&tmB, &full_bar[stage], sB, kb * GEMM_BK, n_blk * BN);
-          } else {
-#pragma unroll
-            for (int a = 0; a < BN / 64; ++a)
-              tma_load_2d(&tmB, &full_bar[stage], sB + a * (GEMM_BK * 128), n_blk * BN + a * 64, kb * GEMM_BK);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
+        const auto w = sched.work(item, 0);
+        for (int kb = w.kb0; kb < w.kb1; ++kb)
+          gemm_fill<Cfg, A_MN, B_MN, 1, false>(smem, full_bar, empty_bar, ring, &tmA, nullptr, &tmB, p, kb, w.m_blk, w.n_blk, 0);
       }
     }
   } else {
@@ -813,47 +832,13 @@ gemm_sm90_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     uint8_t* sw = staging + (4 * cw + quad) * 4096;
     // this warpgroup's 128 rows of A: 128 rows further down (K-major) or the third and fourth 64-wide MN blocks; 16 KB either way
     const uint32_t a_half = (uint32_t)cw * (A_MN ? 2 * GEMM_BK * 128 : 128 * 128);
-    int stage = 0; uint32_t phase = 0;
+    GemmRing<STAGES> ring;
     auto release = [&](int s) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[s]); };
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      const int split = item / tiles;
-      const int rem = item - split * tiles;
-      const int m_blk = rem / n_tiles, n_blk = rem - m_blk * n_tiles;
-      const int kb0 = split * kb_per_split;
-      const int kb1 = min(kb0 + kb_per_split, kb_total);
+      const auto [m_blk, n_blk, kb0, kb1] = sched.work(item, 0);
       float d0[64], d1[64];                                   // accumulator rows 0-63 / 64-127 of this warpgroup's half
-#pragma unroll
-      for (int i = 0; i < 64; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
-      int prev_stage = -1;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES) + a_half;
-        const uint32_t sB = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
-        wgmma_reg_fence(d0);
-        wgmma_reg_fence(d1);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BK / GEMM_UK; ++k) {
-          const uint64_t db = B_MN ? wgmma_desc_sw128(sB + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
-                                   : wgmma_desc_sw128(sB + k * (GEMM_UK * 2), 16, 1024);
-          const uint64_t da0 = A_MN ? wgmma_desc_sw128(sA + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
-                                    : wgmma_desc_sw128(sA + k * (GEMM_UK * 2), 16, 1024);
-          const uint64_t da1 = A_MN ? wgmma_desc_sw128(sA + GEMM_BK * 128 + k * (GEMM_UK * 128), GEMM_BK * 128, 1024)
-                                    : wgmma_desc_sw128(sA + 64 * 128 + k * (GEMM_UK * 2), 16, 1024);
-          const uint32_t acc_flag = (kb > kb0 || k > 0) ? 1u : 0u;
-          wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d0, da0, db, acc_flag);
-          wgmma_m64n128_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(d1, da1, db, acc_flag);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                        // the previous k-block's MMAs have retired: its smem slot is free
-        if (prev_stage >= 0) release(prev_stage);
-        prev_stage = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      wgmma_reg_fence(d0);
-      wgmma_reg_fence(d1);
-      if (prev_stage >= 0) release(prev_stage);
+      const int last_stage = gemm_mainloop<Cfg, A_MN, B_MN>(smem, full_bar, ring, a_half, kb0, kb1, d0, d1, release);
+      gemm_drain(d0, d1, last_stage, release);
 
       // ---- epilogue: 32-column slices, fragments -> staging tile -> one row per thread -> store_slice
       const int wrow0 = m_blk * BM + 128 * cw + 16 * quad;
@@ -922,6 +907,25 @@ struct GemmOperand {
   long long ld2 = 0;
 };
 
+// tensor map of operand X (mn rows of depth k): K-major boxes are 64 deep x box_rows, MN-major ones one 64-wide MN block x 64 deep
+inline int make_operand_tmap(CUtensorMap* tm, const GemmOperand& X, long long mn, long long k, int box_rows) {
+  return X.mn_major ? make_tmap_bf16(tm, X.ptr, mn, k, X.ld, GEMM_BK) : make_tmap_bf16(tm, X.ptr, k, mn, X.ld, box_rows);
+}
+
+// launch of a persistent kernel without clusters: one CTA per SM, at most one per work item.  The dynamic shared-memory limit is
+// raised on the kernel's first launch.
+template <class Cfg, auto kern, class... Args>
+int launch_persistent(int items, int num_sms, cudaStream_t stream, const Args&... args) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES) != cudaSuccess) return -2;
+    attr_set = true;
+  }
+  const int grid = items < num_sms ? items : num_sms;
+  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(args...);
+  return cudaGetLastError() == cudaSuccess ? 0 : -3;
+}
+
 // CTA pairing (CL = 2): mode 1 (default) never, 2 every launch, 3 launches with at least 16 k-blocks per work item and two tiles per SM.  Set by
 // tfx_gemm_set_cluster_mode, or once from the environment (TFX_GEMM_CLUSTER).  Off by default: on an H100 (400 W limit) the config-2 step's GEMM
 // time doubled with mode 3 (64 -> 129 ms per step, same machine, alternated runs).
@@ -960,19 +964,11 @@ int launch_gemm_wide_t(const GemmOperand& A, const GemmOperand& B, const GemmPar
   const int items = ((p.M + Cfg::BM - 1) / Cfg::BM) * ((p.N + GEMM_BN - 1) / GEMM_BN) * p.k_splits;
   if (items <= 0) return 0;
   CUtensorMap tmA, tmB;
-  int rc = !A_MN ? make_tmap_bf16(&tmA, A.ptr, p.K, p.M, A.ld, Cfg::BM) : make_tmap_bf16(&tmA, A.ptr, p.M, p.K, A.ld, GEMM_BK);
+  int rc = make_operand_tmap(&tmA, A, p.M, p.K, Cfg::BM);
   if (rc) return rc;
-  rc = !B_MN ? make_tmap_bf16(&tmB, B.ptr, p.K, p.N, B.ld, GEMM_BN) : make_tmap_bf16(&tmB, B.ptr, p.N, p.K, B.ld, GEMM_BK);
+  rc = make_operand_tmap(&tmB, B, p.N, p.K, GEMM_BN);
   if (rc) return rc;
-  auto kern = gemm_sm90_wide_kernel<A_MN, B_MN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES) != cudaSuccess) return -2;
-    attr_set = true;
-  }
-  const int grid = items < num_sms ? items : num_sms;
-  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-  return cudaGetLastError() == cudaSuccess ? 0 : -3;
+  return launch_persistent<Cfg, gemm_sm90_wide_kernel<A_MN, B_MN>>(items, num_sms, stream, tmA, tmB, p);
 }
 
 template <bool A_MN, bool B_MN, int EPI>
@@ -980,10 +976,9 @@ int launch_gemm_t(const GemmOperand& A, const GemmOperand& B, const GemmParams& 
   using Cfg = GemmCfg<EPI>;
   GemmParams p = p_in;
   CUtensorMap tmA, tmA2, tmB;
-  int rc;
   const bool two = (!A_MN) && A.ptr2 != nullptr;
   if (!two) p.K1 = p.K;
-  if (!A_MN) rc = make_tmap_bf16(&tmA, A.ptr, two ? p.K1 : p.K, p.M, A.ld, GEMM_BM); else rc = make_tmap_bf16(&tmA, A.ptr, p.M, p.K, A.ld, GEMM_BK);
+  int rc = make_operand_tmap(&tmA, A, p.M, p.K1, GEMM_BM);         // the first K segment (all of K unless A is split)
   if (rc) return rc;
   if (two) { rc = make_tmap_bf16(&tmA2, A.ptr2, p.K - p.K1, p.M, A.ld2, GEMM_BM); if (rc) return rc; } else tmA2 = tmA;
   p.k_splits = gemm_effective_splits(p.K, p.k_splits);
@@ -994,7 +989,7 @@ int launch_gemm_t(const GemmOperand& A, const GemmOperand& B, const GemmParams& 
   const int kb_item = gemm_kb_per_item(p.K, p.k_splits);      // k-blocks per work item
   const bool paired = mode == 2 || (mode == 3 && m_tiles >= 2 && kb_item >= 16 && items >= 2 * num_sms);
   // paired CTAs each fetch half of the B tile: the K-major box is 64 rows (the MN-major box is one 64-wide block either way)
-  if (!B_MN) rc = make_tmap_bf16(&tmB, B.ptr, p.K, p.N, B.ld, paired ? GEMM_BN / 2 : GEMM_BN); else rc = make_tmap_bf16(&tmB, B.ptr, p.N, p.K, B.ld, GEMM_BK);
+  rc = make_operand_tmap(&tmB, B, p.N, p.K, paired ? GEMM_BN / 2 : GEMM_BN);
   if (rc) return rc;
   if (paired) {
     auto kern = gemm_sm90_kernel<A_MN, B_MN, EPI, 2>;
@@ -1017,15 +1012,7 @@ int launch_gemm_t(const GemmOperand& A, const GemmOperand& B, const GemmParams& 
     cfg.gridDim = dim3(2 * clusters);
     return cudaLaunchKernelEx(&cfg, kern, tmA, tmA2, tmB, p) == cudaSuccess ? 0 : -3;
   }
-  auto kern = gemm_sm90_kernel<A_MN, B_MN, EPI, 1>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES) != cudaSuccess) return -2;
-    attr_set = true;
-  }
-  const int grid = items < num_sms ? items : num_sms;
-  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmA2, tmB, p);
-  return cudaGetLastError() == cudaSuccess ? 0 : -3;
+  return launch_persistent<Cfg, gemm_sm90_kernel<A_MN, B_MN, EPI, 1>>(items, num_sms, stream, tmA, tmA2, tmB, p);
 }
 
 }  // namespace tfx
