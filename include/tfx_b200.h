@@ -70,6 +70,14 @@ int tfx_gemm_qkvg(const void* u, long long ldu, const void* W, long long ldw, in
  * mix_pre and the kv_rows append are those of tfx_gemm_qkvg (same accumulators, bit for bit). */
 int tfx_gemm_qkvg_rope(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates,
                        const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream);
+/* dim_head = 128 forms of the two: W = [to_qk | to_v | to_gates | pad], N = 3*H*128 + 128, one head per 128-column tile, so 1 <= H <= 16 (odd H too).
+ * The qk-RMSNorm spans the head's 128 columns (scale sqrt(128)); RoPE takes 64 frequency pairs: rope_cs_t is [64][rope_len][2] (tfx_rope_table, n_freqs 64);
+ * qk_inv is [M][2H] as above; q, k, v are [M][H*128]; gates are rows [3*H*128, +H) of W as in the 64-wide forms, the mix_pre rows start at the next
+ * even row, 3*H*128 + H rounded up to even (so that an odd H keeps the bf16 pairs of their gradient 4-byte aligned). */
+int tfx_gemm_qkvg_d128(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates, float* qk_inv,
+                       const float* q_gamma, const float* k_gamma, const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream);
+int tfx_gemm_qkvg_rope_d128(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates,
+                            const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream);
 
 /* branch output projection + AdaptiveWrapper output gate + residual:
  *   y = [A | A2] W^T + bias ;  x_out = x_res + y * (cond_row[m] >= 0 ? zgate[cond_row[m]] : layerscale + 1)
@@ -115,6 +123,15 @@ int tfx_attn_bwd_tc(const void* q, const void* k, const void* v, const void* do_
                     const float* lse, const float* dsum_hm, const int* kv_limit, const int* kt_kv0, const int* kt_kvend, const int* kt_q0, const int* kt_qend,
                     const int* kt_order /* optional: key-tile indices, most query tiles first (load balance of the persistent grid) */,
                     int n_kv_tiles, float* dq, float* dk, void* dv, long long ld_dv, int M, int H, float scale, float softcap, const float* fast_params, void* stream);
+/* dim_head = 128 forms of tfx_attn_fwd / tfx_attn_bwd_prep / tfx_attn_bwd: the same tile tables, span mask, soft-cap, gates and buffer layouts with
+ * 128-wide heads ([M][H*128]); no bounded-logit variant exists at this head dim, so there is no skip flag.  dq must be zero on entry of the backward. */
+int tfx_attn_fwd_d128(const void* q, const void* k, const void* v, long long ld_q, long long ld_k, long long ld_v, const float* gates, int H,
+                      const int* kv_limit, const int* tile_q0, const int* tile_qend, const int* tile_kv0, const int* tile_kvend, int n_tiles,
+                      void* o, long long ld_o, float* lse, int M, float scale, float softcap, void* stream);
+int tfx_attn_bwd_prep_d128(const void* do_gated, const void* o_gated, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream);
+int tfx_attn_bwd_d128(const void* q, const void* k, const void* v, const void* do_pre, long long ld_q, long long ld_k, long long ld_v, long long ld_do,
+                      const float* lse, const float* dsum_hm, const int* kv_limit, const int* kt_kv0, const int* kt_kvend, const int* kt_q0, const int* kt_qend,
+                      int n_kv_tiles, float* dq, float* dk, void* dv, long long ld_dv, int M, int H, float scale, float softcap, void* stream);
 /* backward of the qk-RMSNorm + RoPE epilogue; packs d[q | k | (v written by attn_bwd) | gates] bf16 [M][out_ld] */
 int tfx_qk_bwd_pack(const float* dq, const float* dk, const void* q_bf16, const void* k_bf16, const float* qk_inv, const float* q_gamma, const float* k_gamma,
                     const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16, long long out_ld,
@@ -124,6 +141,12 @@ int tfx_qk_bwd_pack(const float* dq, const float* dk, const void* q_bf16, const 
  * tfx_qk_bwd_pack, packed into the same d[q | k | . | gates] layout */
 int tfx_qk_bwd_pack_rope(const float* dq, const float* dk, const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16,
                          long long out_ld, int M, int H, void* stream);
+/* dim_head = 128 forms of the two packs (1 <= H <= 16): rope_cs is [rope_len][64][2], the gammas are [128], the norm scale is sqrt(128) */
+int tfx_qk_bwd_pack_d128(const float* dq, const float* dk, const void* q_bf16, const void* k_bf16, const float* qk_inv, const float* q_gamma, const float* k_gamma,
+                         const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16, long long out_ld,
+                         float* dq_gamma, float* dk_gamma, int M, int H, void* stream);
+int tfx_qk_bwd_pack_rope_d128(const float* dq, const float* dk, const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16,
+                              long long out_ld, int M, int H, void* stream);
 
 /* AttentionResidual backward with DEFERRED assembly (exact; rowops.cu): instead of read-modify-writing the gradient of every earlier hidden at every layer, layer i
  * stores three scalars per (token, hidden) and the complete gradient of ONE hidden is assembled when the backward pass needs it:
@@ -152,6 +175,13 @@ int tfx_vmix_fwd(void* v_inout, long long ld_v, const int* rows, const void* v_f
 int tfx_vmix_bwd(void* dv_inout, long long ld_dv, const void* v_mixed, long long ld_v, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias,
                  float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream);
 int tfx_add_f32_into_bf16(void* dst_bf16, long long ld_dst, const float* src, long long ld_src, int M, int N, void* stream);
+/* dim_head = 128 forms of the per-head row kernels (heads of 128 columns).  tfx_laser_v_fwd / tfx_laser_v_bwd are elementwise: at dim_head = 128 they
+ * are called with 2H 64-wide heads. */
+int tfx_laser_out_fwd_d128(const void* o_laser, const float* gates, void* att, int M, int H, void* stream);
+int tfx_laser_bwd_prep_d128(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream);
+int tfx_vmix_fwd_d128(void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias, int M, int H, void* stream);
+int tfx_vmix_bwd_d128(void* dv_inout, long long ld_dv, const void* v_mixed, long long ld_v, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias,
+                      float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream);
 
 /* ---------------------------------------------------------------- warp-per-token kernels (D = model dim: 128, 256, 384, 512, 768 or 1024)
  * AdaptiveWrapper input side (T.py:747-755, text-only 677-679): u = isM ? LN(x)(gamma_c+1)+beta_c : LN(x)(g+1).
@@ -263,6 +293,9 @@ int tfx_decode_prep(const int* state, int S, int cap, int slab0, int* text_id, i
  * [tile_kv0, min(tile_kvend, kv_limit[row]+1)) of the cache; soft-cap, softmax, value gate as tfx_attn_fwd. */
 int tfx_attn_decode(const void* q, const void* k, const void* v, long long ld_q, long long ld_k, long long ld_v, const float* gates, int H, const int* kv_limit,
                     const int* tile_q0, const int* tile_kv0, const int* tile_kvend, int n_tiles, void* o, long long ld_o, float scale, float softcap, void* stream);
+/* the same at dim_head = 128 (q, k, v, o rows of H*128) */
+int tfx_attn_decode_d128(const void* q, const void* k, const void* v, long long ld_q, long long ld_k, long long ld_v, const float* gates, int H, const int* kv_limit,
+                         const int* tile_q0, const int* tile_kv0, const int* tile_kvend, int n_tiles, void* o, long long ld_o, float scale, float softcap, void* stream);
 /* token sampling + state update for every sample in the text phase (sample_text_token T.py:580-591; greedy / gumbel of generate_text_only
  * T.py:2692-2698 with vlimit = num_text_tokens; bookkeeping T.py:2330-2349).  rows (optional): logits row of sample s (first token after the
  * prefill, taken at the last prompt position, T.py:2225-2250: advance = 0 - that token only gets its cache row on the next step).

@@ -25,6 +25,8 @@ SIGNATURES = {
     'tfx_gemm_store': [VP, LL, I, VP, LL, I, I, I, I, VP, LL, VP, LL, VP, VP, F, I, I, VP],
     'tfx_gemm_qkvg': [VP, LL, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP],
     'tfx_gemm_qkvg_rope': [VP, LL, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, I, VP, VP, VP],
+    'tfx_gemm_qkvg_d128': [VP, LL, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP],
+    'tfx_gemm_qkvg_rope_d128': [VP, LL, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, I, VP, VP, VP],
     'tfx_gemm_resid': [VP, LL, VP, LL, I, VP, LL, I, I, I, VP, VP, VP, VP, VP, VP, VP, LL, VP, VP],
     'tfx_gemm_geglu': [VP, LL, VP, LL, VP, I, I, I, VP, VP, VP],
     'tfx_gemm_geglu_drop': [VP, LL, VP, LL, VP, I, I, I, VP, VP, VP, F, I, VP],
@@ -34,8 +36,13 @@ SIGNATURES = {
     'tfx_attn_bwd_prep': [VP, VP, VP, VP, VP, VP, VP, I, I, VP],
     'tfx_attn_bwd': [VP, VP, VP, VP, LL, LL, LL, LL, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP, LL, I, I, F, F, VP, VP],
     'tfx_attn_bwd_tc': [VP, VP, VP, VP, LL, LL, LL, LL, VP, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP, LL, I, I, F, F, VP, VP],
+    'tfx_attn_fwd_d128': [VP, VP, VP, LL, LL, LL, VP, I, VP, VP, VP, VP, VP, I, VP, LL, VP, I, F, F, VP],
+    'tfx_attn_bwd_prep_d128': [VP, VP, VP, VP, VP, VP, VP, I, I, VP],
+    'tfx_attn_bwd_d128': [VP, VP, VP, VP, LL, LL, LL, LL, VP, VP, VP, VP, VP, VP, VP, I, VP, VP, VP, LL, I, I, F, F, VP],
     'tfx_qk_bwd_pack': [VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, LL, VP, VP, I, I, VP],
     'tfx_qk_bwd_pack_rope': [VP, VP, VP, VP, VP, VP, VP, LL, I, I, VP],
+    'tfx_qk_bwd_pack_d128': [VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP, LL, VP, VP, I, I, VP],
+    'tfx_qk_bwd_pack_rope_d128': [VP, VP, VP, VP, VP, VP, VP, LL, I, I, VP],
     'tfx_adaln_fwd': [VP, VP, VP, LL, VP, VP, VP, I, I, VP],
     'tfx_adaln_bwd': [VP, VP, VP, VP, VP, LL, VP, VP, VP, LL, VP, I, I, VP],
     'tfx_resid_bwd': [VP, VP, VP, VP, LL, VP, VP, VP, LL, VP, VP, I, I, VP],
@@ -68,6 +75,7 @@ SIGNATURES = {
     'tfx_adam_step': [VP, VP, VP, VP, LL, F, F, F, F, F, I, I, F, I, VP, VP],
     'tfx_decode_prep': [VP, I, I, I, VP, VP, VP, VP, VP, VP, VP, VP, VP, VP],
     'tfx_attn_decode': [VP, VP, VP, LL, LL, LL, VP, I, VP, VP, VP, VP, I, VP, LL, F, F, VP],
+    'tfx_attn_decode_d128': [VP, VP, VP, LL, LL, LL, VP, I, VP, VP, VP, VP, I, VP, LL, F, F, VP],
     'tfx_sample_tokens': [VP, LL, VP, I, I, VP, I, VP, I, I, VP, I, I, F, F, ULL, VP, I, VP],
     'tfx_ode_pre': [VP, VP, VP, LL, I, VP, VP, VP, I, VP],
     'tfx_ode_post': [VP, VP, VP, VP, F, LL, VP, VP, VP],
@@ -81,6 +89,10 @@ SIGNATURES = {
     'tfx_vmix_fwd': [VP, LL, VP, VP, LL, VP, VP, I, I, VP],
     'tfx_vmix_bwd': [VP, LL, VP, LL, VP, LL, VP, VP, VP, VP, LL, I, I, VP],
     'tfx_add_f32_into_bf16': [VP, LL, VP, LL, I, I, VP],
+    'tfx_laser_out_fwd_d128': [VP, VP, VP, I, I, VP],
+    'tfx_laser_bwd_prep_d128': [VP, VP, VP, VP, VP, VP, VP, I, I, VP],
+    'tfx_vmix_fwd_d128': [VP, LL, VP, VP, LL, VP, VP, I, I, VP],
+    'tfx_vmix_bwd_d128': [VP, LL, VP, LL, VP, LL, VP, VP, VP, VP, LL, I, I, VP],
 }
 
 EXPORTED = ['tfx_last_error', 'tfx_version', 'tfx_geglu_bwd_rows_per_block', 'tfx_attn_residual_bwd_workspace_floats', 'tfx_rep_cos_blocks'] + list(SIGNATURES)

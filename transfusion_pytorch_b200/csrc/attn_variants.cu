@@ -165,6 +165,118 @@ __global__ void __launch_bounds__(ROW_THREADS) vmix_bwd_k(__nv_bfloat16* __restr
   }
 }
 
+// ---- head dim 128 (templates instantiated at 128 only; the 64-wide kernels above keep their own code): DH / 8 lanes per head (16 at 128),
+// 32 / (DH / 8) heads per pass.  laser_v_fwd / laser_v_bwd are elementwise and serve any head dim (a 128-wide head is two 64-wide ones).
+#define VAR_ROW_LOOP_DH                                                                                \
+  constexpr int LPH = DH / 8, HPP = 32 / LPH;                                                          \
+  const int lane = threadIdx.x & 31, sub = lane % LPH, hq = lane / LPH;                                \
+  const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5; \
+  for (int row = warp0; row < M; row += nwarps)                                                        \
+    for (int h0 = 0; h0 < H; h0 += HPP)
+
+template <int LPH>
+__device__ __forceinline__ float sum_head_lanes(float s) {
+#pragma unroll
+  for (int o = 1; o < LPH; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  return s;
+}
+
+template <int DH>
+__global__ void __launch_bounds__(ROW_THREADS) laser_out_fwd_dh_k(const __nv_bfloat16* __restrict__ o, const float* __restrict__ gates, __nv_bfloat16* __restrict__ att, int M, int H) {
+  const long long HI = (long long)H * DH;
+  VAR_ROW_LOOP_DH {
+    const int h = h0 + hq;
+    if (h >= H) continue;
+    const long long off = row * HI + h * DH + sub * 8;
+    const float sg = gates ? sigmoid_v(gates[(long long)row * H + h]) : 1.f;
+    float x[8];
+    ld8(o + off, x);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) x[e] = __logf(fmaxf(x[e], 1e-30f)) * sg;
+    st8(att + off, x);
+  }
+}
+
+template <int DH>
+__global__ void __launch_bounds__(ROW_THREADS) laser_bwd_prep_dh_k(const __nv_bfloat16* __restrict__ datt, const __nv_bfloat16* __restrict__ o, const float* __restrict__ gates,
+                                                                  __nv_bfloat16* __restrict__ dop, float* __restrict__ dsum, float* __restrict__ dsum_rowmajor,
+                                                                  float* __restrict__ dq_zero, int M, int H) {
+  const long long HI = (long long)H * DH;
+  VAR_ROW_LOOP_DH {
+    const int h = h0 + hq;
+    const bool act = h < H;
+    const long long off = row * HI + (act ? h : 0) * DH + sub * 8;
+    const float sg = (act && gates) ? sigmoid_v(gates[(long long)row * H + h]) : 1.f;
+    float a[8], b[8], w[8];
+    ld8(datt + off, a); ld8(o + off, b);
+    float s = 0.f, gsum = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float oo = fmaxf(b[e], 1e-30f);
+      s += a[e] * sg;
+      gsum += a[e] * __logf(oo) * sg;
+      w[e] = a[e] * sg / oo;
+    }
+    s = sum_head_lanes<LPH>(s); gsum = sum_head_lanes<LPH>(gsum);
+    if (act) {
+      st8(dop + off, w);
+      if (sub == 0) { dsum[(long long)h * M + row] = s; if (dsum_rowmajor) dsum_rowmajor[(long long)row * H + h] = gsum; }
+      if (dq_zero) {
+        *reinterpret_cast<float4*>(dq_zero + off) = make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(dq_zero + off + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    }
+  }
+}
+
+template <int DH>
+__global__ void __launch_bounds__(ROW_THREADS) vmix_fwd_dh_k(__nv_bfloat16* __restrict__ v, long long ld_v, const int* __restrict__ rows, const __nv_bfloat16* __restrict__ v0,
+                                                            long long ld_v0, const float* __restrict__ mixpre, const float* __restrict__ bias, int M, int H) {
+  VAR_ROW_LOOP_DH {
+    const int h = h0 + hq;
+    if (h >= H) continue;
+    const long long r = rows ? rows[row] : row;
+    const float mix = sigmoid_v(mixpre[(long long)row * H + h] + bias[h]);
+    float a[8], b[8];
+    ld8(v + r * ld_v + h * DH + sub * 8, a); ld8(v0 + r * ld_v0 + h * DH + sub * 8, b);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) a[e] = a[e] * mix + b[e] * (1.f - mix);
+    st8(v + r * ld_v + h * DH + sub * 8, a);
+  }
+}
+
+template <int DH>
+__global__ void __launch_bounds__(ROW_THREADS) vmix_bwd_dh_k(__nv_bfloat16* __restrict__ dv, long long ld_dv, const __nv_bfloat16* __restrict__ vm, long long ld_v,
+                                                            const __nv_bfloat16* __restrict__ v0, long long ld_v0, const float* __restrict__ mixpre, const float* __restrict__ bias,
+                                                            float* __restrict__ dv0_acc, __nv_bfloat16* __restrict__ dmix, long long ld_dmix, int M, int H) {
+  const long long HI = (long long)H * DH;
+  VAR_ROW_LOOP_DH {
+    const int h = h0 + hq;
+    const bool act = h < H;
+    const int hh = act ? h : 0;
+    const float mix = sigmoid_v(mixpre[(long long)row * H + hh] + bias[hh]);
+    float g[8], a[8], b[8];
+    ld8(dv + (long long)row * ld_dv + hh * DH + sub * 8, g);
+    ld8(vm + (long long)row * ld_v + hh * DH + sub * 8, a);
+    ld8(v0 + (long long)row * ld_v0 + hh * DH + sub * 8, b);
+    float s = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) s += g[e] * (a[e] - b[e]);
+    s = sum_head_lanes<LPH>(s) * (1.f - mix);
+    if (act) {
+      float* acc = dv0_acc + row * HI + h * DH + sub * 8;
+      const float4 c0 = *reinterpret_cast<const float4*>(acc), c1 = *reinterpret_cast<const float4*>(acc + 4);
+      const float om = 1.f - mix;
+      *reinterpret_cast<float4*>(acc) = make_float4(c0.x + g[0] * om, c0.y + g[1] * om, c0.z + g[2] * om, c0.w + g[3] * om);
+      *reinterpret_cast<float4*>(acc + 4) = make_float4(c1.x + g[4] * om, c1.y + g[5] * om, c1.z + g[6] * om, c1.w + g[7] * om);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) g[e] *= mix;
+      st8(dv + (long long)row * ld_dv + h * DH + sub * 8, g);
+      if (sub == 0) dmix[(long long)row * ld_dmix + h] = __float2bfloat16(s);
+    }
+  }
+}
+
 // dst(bf16) += src(fp32): first-layer value gradient += what the later layers' value residuals sent back
 __global__ void __launch_bounds__(ROW_THREADS) add_f32_into_bf16_k(__nv_bfloat16* __restrict__ dst, long long ld_dst, const float* __restrict__ src, long long ld_src, int M, int N) {
   const int per_row = N / 8;
@@ -233,6 +345,34 @@ int tfx_vmix_bwd(void* dv_inout, long long ld_dv, const void* v_mixed, long long
   TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && ld_dv % 8 == 0, "vmix_bwd: row pitches must be multiples of 8 bf16");
   vmix_bwd_k<<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc, BF(dmix_bf16), ld_dmix, M, H);
   return check_launch("vmix_bwd");
+}
+
+int tfx_laser_out_fwd_d128(const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  laser_out_fwd_dh_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
+  return check_launch("laser_out_fwd_d128");
+}
+
+int tfx_laser_bwd_prep_d128(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  laser_bwd_prep_dh_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
+  return check_launch("laser_bwd_prep_d128");
+}
+
+int tfx_vmix_fwd_d128(void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias, int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && mix_pre && mix_bias, "vmix_fwd_d128: bad arguments");
+  vmix_fwd_dh_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
+  return check_launch("vmix_fwd_d128");
+}
+
+int tfx_vmix_bwd_d128(void* dv_inout, long long ld_dv, const void* v_mixed, long long ld_v, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias,
+                      float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && ld_dv % 8 == 0, "vmix_bwd_d128: row pitches must be multiples of 8 bf16");
+  vmix_bwd_dh_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc,
+                                                                 BF(dmix_bf16), ld_dmix, M, H);
+  return check_launch("vmix_bwd_d128");
 }
 
 int tfx_add_f32_into_bf16(void* dst_bf16, long long ld_dst, const float* src, long long ld_src, int M, int N, void* stream) {

@@ -106,6 +106,82 @@ __global__ void __launch_bounds__(128) attn_decode_k(const __nv_bfloat16* __rest
   }
 }
 
+// head dim 128 (template, instantiated at 128 only; the 64-wide kernel above keeps its own code): lane <-> DH / 32 output dims for P V
+template <int DH>
+__global__ void __launch_bounds__(128) attn_decode_dh_k(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k, const __nv_bfloat16* __restrict__ v,
+                                                       long long ld_q, long long ld_k, long long ld_v, const float* __restrict__ gates, int H, const int* __restrict__ kv_limit,
+                                                       const int* __restrict__ tile_q0, const int* __restrict__ tile_kv0, const int* __restrict__ tile_kvend,
+                                                       __nv_bfloat16* __restrict__ o, long long ld_o, float scale, float cap) {
+  constexpr int NV = DH / 32;
+  static_assert(NV == 4, "the P V loop and the output store move 4 dims per lane");
+  __shared__ float sq[DH];
+  __shared__ float s_m[4], s_l[4];
+  __shared__ float s_o[4][DH];
+  const int tile = blockIdx.x, head = blockIdx.y;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int row = tile_q0[tile];
+  const int kv0 = tile_kv0[tile];
+  const int kv_end = min(tile_kvend[tile], kv_limit[row] + 1);
+  if (tid < DH) sq[tid] = __bfloat162float(q[(long long)row * ld_q + head * DH + tid]) * scale;
+  __syncthreads();
+  const float inv_cap = 1.f / cap;
+  float m = -INFINITY, l = 0.f, a[NV];
+#pragma unroll
+  for (int e = 0; e < NV; ++e) a[e] = 0.f;
+  for (int base = kv0 + warp * 32; base < kv_end; base += 128) {
+    const int key = base + lane;
+    const bool ok = key < kv_end;
+    float s = -INFINITY;
+    if (ok) {
+      const uint4* kp = reinterpret_cast<const uint4*>(k + (long long)key * ld_k + head * DH);
+      float d = 0.f;
+#pragma unroll
+      for (int c = 0; c < DH / 8; ++c) {
+        const uint4 t = kp[c];
+        const float2 x0 = unpack2_bf16(t.x), x1 = unpack2_bf16(t.y), x2 = unpack2_bf16(t.z), x3 = unpack2_bf16(t.w);
+        d += x0.x * sq[c * 8] + x0.y * sq[c * 8 + 1] + x1.x * sq[c * 8 + 2] + x1.y * sq[c * 8 + 3] + x2.x * sq[c * 8 + 4] + x2.y * sq[c * 8 + 5] +
+             x3.x * sq[c * 8 + 6] + x3.y * sq[c * 8 + 7];
+      }
+      s = cap * tanh_acc_d(d * inv_cap);
+    }
+    const float mn = fmaxf(m, warp_max(s));            // finite: lane 0 of this chunk is a valid key
+    const float p = ok ? __expf(s - mn) : 0.f;
+    const float corr = __expf(m - mn);
+    l = l * corr + warp_sum(p);
+#pragma unroll
+    for (int e = 0; e < NV; ++e) a[e] *= corr;
+    m = mn;
+    const int nk = min(32, kv_end - base);
+#pragma unroll 4
+    for (int j = 0; j < nk; ++j) {
+      const float pj = __shfl_sync(0xffffffffu, p, j);
+      const uint2 w = *reinterpret_cast<const uint2*>(v + (long long)(base + j) * ld_v + head * DH + NV * lane);
+      const float2 v0 = unpack2_bf16(w.x), v1 = unpack2_bf16(w.y);
+      a[0] = fmaf(pj, v0.x, a[0]); a[1] = fmaf(pj, v0.y, a[1]); a[2] = fmaf(pj, v1.x, a[2]); a[3] = fmaf(pj, v1.y, a[3]);
+    }
+  }
+  if (lane == 0) { s_m[warp] = m; s_l[warp] = l; }
+#pragma unroll
+  for (int e = 0; e < NV; ++e) s_o[warp][NV * lane + e] = a[e];
+  __syncthreads();
+  if (warp == 0) {
+    float M4 = fmaxf(fmaxf(s_m[0], s_m[1]), fmaxf(s_m[2], s_m[3]));
+    float L = 0.f, out[NV];
+#pragma unroll
+    for (int e = 0; e < NV; ++e) out[e] = 0.f;
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      const float c = s_m[w] == -INFINITY ? 0.f : __expf(s_m[w] - M4);
+      L += s_l[w] * c;
+#pragma unroll
+      for (int e = 0; e < NV; ++e) out[e] += s_o[w][NV * lane + e] * c;
+    }
+    float g = L > 0.f ? 1.f / L : 0.f;
+    if (gates) g *= 1.f / (1.f + __expf(-gates[(long long)row * H + head]));
+    *reinterpret_cast<uint2*>(o + (long long)row * ld_o + head * DH + NV * lane) = make_uint2(pack2_bf16(out[0] * g, out[1] * g), pack2_bf16(out[2] * g, out[3] * g));
+  }
+}
+
 __device__ __forceinline__ unsigned long long mix64(unsigned long long z) {
   z += 0x9E3779B97F4A7C15ull;
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
@@ -228,6 +304,16 @@ int tfx_attn_decode(const void* q, const void* k, const void* v, long long ld_q,
   attn_decode_k<<<dim3(n_tiles, H), 128, 0, ST(stream)>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, ld_q, ld_k, ld_v, gates, H, kv_limit, tile_q0,
                                                          tile_kv0, tile_kvend, (__nv_bfloat16*)o, ld_o, scale, softcap);
   return check_launch("attn_decode");
+}
+
+int tfx_attn_decode_d128(const void* q, const void* k, const void* v, long long ld_q, long long ld_k, long long ld_v, const float* gates, int H, const int* kv_limit,
+                         const int* tile_q0, const int* tile_kv0, const int* tile_kvend, int n_tiles, void* o, long long ld_o, float scale, float softcap, void* stream) {
+  if (n_tiles <= 0) return 0;
+  TFX_REQUIRE(softcap > 0.f, "attn_decode_d128: softcap must be > 0 (got %f)", softcap);
+  TFX_REQUIRE(ld_k % 8 == 0 && ld_v % 4 == 0 && ld_o % 4 == 0, "attn_decode_d128: row pitches must keep 16-byte key rows and 8-byte value / output quads aligned");
+  attn_decode_dh_k<128><<<dim3(n_tiles, H), 128, 0, ST(stream)>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, ld_q, ld_k, ld_v, gates, H, kv_limit,
+                                                                 tile_q0, tile_kv0, tile_kvend, (__nv_bfloat16*)o, ld_o, scale, softcap);
+  return check_launch("attn_decode_d128");
 }
 
 int tfx_sample_tokens(const float* logits, long long ld_logits, const int* rows, int V, int vlimit, int* state, int S, int* hist, int hist_cap, int eos_id, const int* som_ids,

@@ -102,6 +102,33 @@ int tfx_gemm_qkvg_rope(const void* u, long long ldu, const void* W, long long ld
   return finish(launch_gemm_t<false, false, EPI_QKVG_ROPE>(a, b, p, num_sms(), ST(stream)), "gemm_qkvg_rope");
 }
 
+// head dim 128: W is [to_qk | to_v | to_gates | pad] with N = 3 H 128 + 128; one head per 128-column tile, so any H in [1, 16]
+int tfx_gemm_qkvg_d128(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates, float* qk_inv,
+                       const float* q_gamma, const float* k_gamma, const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(H >= 1 && H <= 16, "gemm_qkvg_d128: heads must be in [1, 16] (got %d)", H);
+  TFX_REQUIRE(ldu % 8 == 0 && ldw % 8 == 0, "gemm_qkvg_d128: row pitches must be multiples of 8");
+  GemmParams p; memset(&p, 0, sizeof(p));
+  p.M = M; p.N = 3 * H * 128 + 128; p.K = D; p.k_splits = 1; p.H = H;
+  p.q = (__nv_bfloat16*)q; p.k = (__nv_bfloat16*)k; p.v = (__nv_bfloat16*)v; p.gates = gates; p.qk_inv = qk_inv;
+  p.q_gamma = q_gamma; p.k_gamma = k_gamma; p.rope_pos = rope_pos; p.rope_cs = (const float2*)rope_cs_t; p.rope_len = rope_len; p.kv_rows = kv_rows; p.mix_pre = mix_pre;
+  GemmOperand a{u, ldu, false}, b{W, ldw, false};
+  return finish(launch_gemm_t<false, false, EPI_QKVG_D128>(a, b, p, num_sms(), ST(stream)), "gemm_qkvg_d128");
+}
+
+int tfx_gemm_qkvg_rope_d128(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates,
+                            const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(H >= 1 && H <= 16, "gemm_qkvg_rope_d128: heads must be in [1, 16] (got %d)", H);
+  TFX_REQUIRE(ldu % 8 == 0 && ldw % 8 == 0, "gemm_qkvg_rope_d128: row pitches must be multiples of 8");
+  GemmParams p; memset(&p, 0, sizeof(p));
+  p.M = M; p.N = 3 * H * 128 + 128; p.K = D; p.k_splits = 1; p.H = H;
+  p.q = (__nv_bfloat16*)q; p.k = (__nv_bfloat16*)k; p.v = (__nv_bfloat16*)v; p.gates = gates;
+  p.rope_pos = rope_pos; p.rope_cs = (const float2*)rope_cs_t; p.rope_len = rope_len; p.kv_rows = kv_rows; p.mix_pre = mix_pre;
+  GemmOperand a{u, ldu, false}, b{W, ldw, false};
+  return finish(launch_gemm_t<false, false, EPI_QKVG_ROPE_D128>(a, b, p, num_sms(), ST(stream)), "gemm_qkvg_rope_d128");
+}
+
 int tfx_gemm_resid(const void* A, long long lda, const void* A2, long long lda2, int K1, const void* W, long long ldw, int M, int N, int K, const float* bias,
                    const float* x_res, float* x_out, void* x_out_bf16, void* y_bf16, const int* cond_row, const float* zgate, long long zgate_ld,
                    const float* layerscale, void* stream) {

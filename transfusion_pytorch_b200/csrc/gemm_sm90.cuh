@@ -40,7 +40,8 @@ constexpr int GEMM_BK = 64;     // 64 bf16 = 128 B = one swizzle atom row
 constexpr int GEMM_UK = 16;     // wgmma K for 16-bit inputs
 
 // GEGLU_DROP: GEGLU with FFN dropout on h.  QKVG_ROPE: QKVG without the qk-RMSNorm (`qk_rmsnorm = False`): q, k = RoPE(acc), no qk_inv
-enum : int { EPI_STORE = 0, EPI_QKVG = 1, EPI_RESID = 2, EPI_GEGLU = 3, EPI_GEGLU_DROP = 4, EPI_QKVG_ROPE = 5 };
+// QKVG_D128 / QKVG_ROPE_D128: QKVG / QKVG_ROPE at head dim 128 (one head per 128-column tile; rope_cs is [64][rope_len])
+enum : int { EPI_STORE = 0, EPI_QKVG = 1, EPI_RESID = 2, EPI_GEGLU = 3, EPI_GEGLU_DROP = 4, EPI_QKVG_ROPE = 5, EPI_QKVG_D128 = 6, EPI_QKVG_ROPE_D128 = 7 };
 
 struct GemmParams {
   int M, N, K;                 // D is M x N, reduction K
@@ -545,7 +546,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int rows_valid = min(32, p.M - wrow0);            // may be <= 0
       const int col0 = n_blk * BN;
       int qk_pos = 0;
-      if constexpr (EPI == EPI_QKVG || EPI == EPI_QKVG_ROPE) { qk_pos = row_ok ? p.rope_pos[row] : 0; }
+      if constexpr (EPI == EPI_QKVG || EPI == EPI_QKVG_ROPE || EPI == EPI_QKVG_D128 || EPI == EPI_QKVG_ROPE_D128) { qk_pos = row_ok ? p.rope_pos[row] : 0; }
       if constexpr (EPI == EPI_RESID) { qk_pos = (row_ok && p.cond_row) ? p.cond_row[row] : -1; }      // (reused as the condition row)
 
       if constexpr (EPI == EPI_STORE) {
@@ -632,6 +633,89 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               float* dm = p.mix_pre + (long long)row * p.H;
 #pragma unroll
               for (int j = 0; j < 32; ++j) if (j >= p.H && j < 2 * p.H) dm[j - p.H] = __uint_as_float(r[j]);
+            }
+          }
+        }
+      } else if constexpr (EPI == EPI_QKVG_D128 || EPI == EPI_QKVG_ROPE_D128) {
+        // head dim 128: N tile = 1 head (H q tiles | H k tiles | H v tiles | 1 gate tile); the q / k norm spans the whole tile row
+        const int kind = n_blk / p.H;         // 0 q, 1 k, 2 v, 3 gates
+        const int tis = n_blk - kind * p.H;   // tile in section = head
+        const long long HI = (long long)p.H * 128;
+        if (kind <= 1) {
+          const float* gamma = kind == 0 ? p.q_gamma : p.k_gamma;
+          __nv_bfloat16* dstm = kind == 0 ? p.q : p.k;
+          const float2* cs = p.rope_cs + qk_pos;        // entry i of this row's position: cs[i * rope_len]
+          float sc = 1.f;                               // qk-RMSNorm: sqrt(128) / |x| (times gamma + 1 per dim below)
+          if constexpr (EPI == EPI_QKVG_D128) {
+            float ss = 0.f;
+#pragma unroll 1
+            for (int c = 0; c < 4; ++c) {
+              uint32_t r[32];
+              acc_ld32(acc, erow, c * 32, r);
+#pragma unroll
+              for (int j = 0; j < 32; ++j) { const float a = __uint_as_float(r[j]); ss += a * a; }
+            }
+            const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
+            if (row_ok) p.qk_inv[(long long)row * 2 * p.H + kind * p.H + tis] = inv;
+            sc = inv * 11.313708498984761f;
+          }
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {              // the head's two 64-column halves
+            uint32_t r0[32], r1[32];
+            acc_ld32(acc, erow, hh * 64, r0);
+            acc_ld32(acc, erow, hh * 64 + 32, r1);
+            uint32_t outw[32];
+#pragma unroll
+            for (int dh = 0; dh < 2; ++dh) {
+              uint32_t* rr = dh == 0 ? r0 : r1;
+#pragma unroll
+              for (int i = 0; i < 16; ++i) {
+                const int d0 = hh * 64 + dh * 32 + 2 * i;
+                float y0 = __uint_as_float(rr[2 * i]), y1 = __uint_as_float(rr[2 * i + 1]);
+                if constexpr (EPI == EPI_QKVG_D128) {
+                  const float2 gm = *reinterpret_cast<const float2*>(gamma + d0);
+                  y0 = y0 * sc * (gm.x + 1.f);
+                  y1 = y1 * sc * (gm.y + 1.f);
+                }
+                const float2 cc = cs[(long long)(d0 >> 1) * p.rope_len];
+                outw[dh * 16 + i] = pack_bf16(y0 * cc.x - y1 * cc.y, y1 * cc.x + y0 * cc.y);
+              }
+            }
+            stg_put<8>(sw, lane, outw);
+            __syncwarp();
+            if (kind == 1 && p.kv_rows) stg_store_rows<8>(sw, lane, reinterpret_cast<uint8_t*>(dstm + tis * 128 + hh * 64), HI * 2, rows_valid, p.kv_rows + wrow0);
+            else stg_store<8>(sw, lane, reinterpret_cast<uint8_t*>(dstm + (long long)wrow0 * HI + tis * 128 + hh * 64), HI * 2, rows_valid);
+            __syncwarp();
+          }
+        } else if (kind == 2) {
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            uint32_t r0[32], r1[32], w[32];
+            acc_ld32(acc, erow, c * 64, r0);
+            acc_ld32(acc, erow, c * 64 + 32, r1);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              w[j] = pack_bf16(__uint_as_float(r0[2 * j]), __uint_as_float(r0[2 * j + 1]));
+              w[16 + j] = pack_bf16(__uint_as_float(r1[2 * j]), __uint_as_float(r1[2 * j + 1]));
+            }
+            stg_put<8>(sw, lane, w);
+            __syncwarp();
+            if (p.kv_rows) stg_store_rows<8>(sw, lane, reinterpret_cast<uint8_t*>(p.v + tis * 128 + c * 64), HI * 2, rows_valid, p.kv_rows + wrow0);
+            else stg_store<8>(sw, lane, reinterpret_cast<uint8_t*>(p.v + (long long)wrow0 * HI + tis * 128 + c * 64), HI * 2, rows_valid);
+            __syncwarp();
+          }
+        } else {
+          uint32_t r[32];
+          acc_ld32(acc, erow, 0, r);
+          if (row_ok) {
+            float* dst = p.gates + (long long)row * p.H;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) if (j < p.H) dst[j] = __uint_as_float(r[j]);
+            if (p.mix_pre) {                            // mix columns start at an even column (bf16 pairs of their gradient stay 4-byte aligned)
+              const int m0 = (p.H + 1) & ~1;
+              float* dm = p.mix_pre + (long long)row * p.H;
+#pragma unroll
+              for (int j = 0; j < 32; ++j) if (j >= m0 && j < m0 + p.H) dm[j - m0] = __uint_as_float(r[j]);
             }
           }
         }

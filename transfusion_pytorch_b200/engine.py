@@ -30,7 +30,7 @@ from torch import Tensor
 from . import _lib
 from ._pinned import POOL
 from .modality_processing import RaggedBatch
-from .transfusion import MODEL_DIMS, MIN_HEADS, MAX_HEADS
+from .transfusion import MODEL_DIMS, MIN_HEADS, MAX_HEADS, DIM_HEADS, MAX_HEADS_D128
 
 BF16, F32, I32, I64 = torch.bfloat16, torch.float32, torch.int32, torch.int64
 
@@ -125,7 +125,7 @@ def wgrad_splits(n_out, n_in, K, sms):
 
 class KVCache:
     """Slab kv cache (decode path; reference layout `(layers, 2, batch, heads, seq, dim_head)`, T.py:976-977, 1264, 2260, re-padded and
-    concatenated per step there).  Here: per layer one K (post-RoPE) and one V matrix, bf16 `[n_slabs * cap, heads * 64]`, token-major like
+    concatenated per step there).  Here: per layer one K (post-RoPE) and one V matrix, bf16 `[n_slabs * cap, heads * dim_head]`, token-major like
     every other activation; sample / branch `s` owns rows `[s * cap, (s + 1) * cap)`.  Appends happen in place from the QKVG GEMM epilogue;
     how much of a slab is valid is host / device bookkeeping of the sampler (`len`), never a mask tensor."""
 
@@ -149,10 +149,14 @@ class Engine:
         self.model = model
         tr = model.transformer
         self.D, self.H, self.depth = tr.dim, tr.heads, tr.depth
-        self.HI = self.H * 64
+        self.DH = tr.dim_head
+        self.HI = self.H * self.DH
         self.inner = tr.ff_inner
         self.Ip = _round_up(self.inner, 64)
         self.NQ = 3 * self.HI + 128                 # packed rows of [to_qk | to_v | to_gates | pad]
+        # first packed row of the value-residual mix Linear (in the pad): right behind the gates, at an even row so that the bf16 pairs of
+        # its gradient columns stay 4-byte aligned (an odd head count exists at dim_head 128 only)
+        self.MIX = 3 * self.HI + _round_up(self.H, 2)
         self.V = model.text_embed.weight.shape[0]
         self.Vp = _round_up(self.V, 8)
         self.Kt = _round_up(self.D + 1, 64)         # padded K of the time-cond Linear
@@ -162,14 +166,25 @@ class Engine:
         # qk_rmsnorm = False (T.py:949-951 skipped): q, k are RoPE(u W^T) only, so no bound on the logits follows from the gammas and every layer runs
         # the general (running-maximum) attention kernels; the q / k norm gammas stay out of the flat buffers (their .grad stays None, as in the reference)
         self.qk_norm = bool(getattr(tr, 'qk_rmsnorm', True))
-        self.fastp = None                           # per layer: bounded-logit attention parameters (tfx_attn_fast_params), qk_rmsnorm models only
+        # the bounded-logit (wgmma) attention kernels exist for 64-wide normed heads only; every other model runs the general kernels alone
+        self.fast = self.qk_norm and self.DH == 64
+        self.fastp = None                           # per layer: bounded-logit attention parameters (tfx_attn_fast_params), `fast` models only
+        # dim_head = 128 takes the `_d128` twin of every per-head kernel (same arguments, 128-wide heads); the elementwise LASER value
+        # kernels see a 128-wide head as two 64-wide ones
+        self.d128 = self.DH == 128
+        self.sfx = '_d128' if self.d128 else ''
+        self.vheads = self.HI // 64
         self.clean, self.clean_eps = bool(getattr(model, 'model_output_clean', False)), float(getattr(model, 'eps', 1e-2))
         self.posemb = tuple(bool(a) for a in getattr(model, 'add_pos_emb', ()))      # per modality type: axial positional embedding on the latent tokens
-        self.scale = 64 ** -0.5
+        self.scale = self.DH ** -0.5
         self.dls = list(model.dim_latents)
         self.dlp = [_round_up(d, 8) for d in self.dls]
         assert self.D in MODEL_DIMS, f'model dim must be one of {MODEL_DIMS} for the row kernels'
-        assert self.H % 2 == 0 and MIN_HEADS <= self.H <= MAX_HEADS, 'heads must be even (two 64-wide heads per 128-column GEMM tile) and at most 32'
+        if self.d128:
+            assert 1 <= self.H <= MAX_HEADS_D128, f'heads must be in [1, {MAX_HEADS_D128}] at dim_head 128'
+        else:
+            assert self.DH == 64, f'dim_head must be one of {DIM_HEADS}'
+            assert self.H % 2 == 0 and MIN_HEADS <= self.H <= MAX_HEADS, 'heads must be even (two 64-wide heads per 128-column GEMM tile) and at most 32'
         self.device = None
         self.flat = None
         self.ws = {}
@@ -266,8 +281,8 @@ class Engine:
             r[:2 * HI] = q_off + np.arange(2 * HI) * D
             r[2 * HI:3 * HI] = v_off + np.arange(HI) * D
             r[3 * HI:3 * HI + H] = g_off + np.arange(H) * D
-            if f'{pre}.1.fn.to_learned_value_residual.0.weight' in self.offs:        # value-residual mix Linear: pad rows [3HI + H, 3HI + 2H) of the packed weight
-                r[3 * HI + H:3 * HI + 2 * H] = self.offs[f'{pre}.1.fn.to_learned_value_residual.0.weight'] + np.arange(H) * D
+            if f'{pre}.1.fn.to_learned_value_residual.0.weight' in self.offs:        # value-residual mix Linear: pad rows [MIX, MIX + H) of the packed weight
+                r[self.MIX:self.MIX + H] = self.offs[f'{pre}.1.fn.to_learned_value_residual.0.weight'] + np.arange(H) * D
             w2_off = self.offs[f'{pre}.2.fn.net.3.weight']
             w2_rows = torch.from_numpy(w2_off + np.arange(D, dtype = np.int64) * inner).to(dev)
             self.layer_maps.append(dict(w1_rows = w1_rows.contiguous(), b1_cols = b1_cols.contiguous(), qkvg_rows = torch.from_numpy(r).to(dev), w2_rows = w2_rows))
@@ -322,7 +337,7 @@ class Engine:
             job(self.P(f'{pre}.1.fn.to_v.0.weight'), D, D, None, wq[2 * HI:], HI, D)
             job(self.P(f'{pre}.1.fn.to_gates.0.weight'), D, D, None, wq[3 * HI:], H, D)
             if f'{pre}.1.fn.to_learned_value_residual.0.weight' in self.named:
-                job(self.P(f'{pre}.1.fn.to_learned_value_residual.0.weight'), D, D, None, wq[3 * HI + H:], H, D)
+                job(self.P(f'{pre}.1.fn.to_learned_value_residual.0.weight'), D, D, None, wq[self.MIX:], H, D)
             job(self.P(f'{pre}.1.fn.to_out.1.weight'), HI, HI, None, dst(f'wo{i}', D, HI), D, HI)
             job(self.P(f'{pre}.2.fn.net.0.weight'), D, D, self.w1_row_src, dst(f'w1{i}', 2 * Ip, D), 2 * Ip, D)
             job(self.P(f'{pre}.2.fn.net.3.weight'), inner, inner, None, dst(f'w2{i}', D, Ip), D, Ip)
@@ -359,7 +374,7 @@ class Engine:
             self._build_pack_jobs()
         self.ops.cast_pack_multi(self._pack_tab, self._pack_blk_job, self._pack_blk_first, self._pack_nblocks)
         # per layer: is the bounded-logit (wgmma) attention path valid for the current q/k norm gammas?  (device-side decision)
-        if self.qk_norm:
+        if self.fast:
             if self.fastp is None or self.fastp.device != self.device:
                 self.fastp = torch.zeros(self.depth, 8, device = self.device, dtype = F32)
             for i in range(self.depth):
@@ -413,15 +428,16 @@ class Engine:
         return rb.dev
 
     def rope_table(self, max_pos: int):
-        """cos/sin tables: [pos][32] (row kernels) and its transpose [32][pos] (thread-per-row QKVG epilogue)"""
+        """cos/sin tables: [pos][dim_head / 2] (row kernels) and its transpose [dim_head / 2][pos] (thread-per-row QKVG epilogue)"""
         n = _round_up(max_pos + 1, 1024)
         t = self.ws.get('rope_cs')
         if t is None or t.shape[0] < n:
             if t is not None and self.graph_pins is not None:
                 self.graph_pins += [t, self.ws['rope_cs_t']]
-            t = torch.empty(n, 32, 2, device = self.device, dtype = F32)
-            tt = torch.empty(32, n, 2, device = self.device, dtype = F32)
-            self.ops.rope_table(self.model.rotary_emb.freqs.detach().float().contiguous(), t, tt, n, 32)
+            nf = self.DH // 2
+            t = torch.empty(n, nf, 2, device = self.device, dtype = F32)
+            tt = torch.empty(nf, n, 2, device = self.device, dtype = F32)
+            self.ops.rope_table(self.model.rotary_emb.freqs.detach().float().contiguous(), t, tt, n, nf)
             self.ws['rope_cs'], self.ws['rope_cs_t'] = t, tt
         return t
 
@@ -559,36 +575,40 @@ class Engine:
             mixpre = self.buf(f'{lt}mix', (M, H), F32) if has_mix else None
             if self.qk_norm:
                 qk_inv = self.buf(f'{lt}qi', (M, 2 * H), F32)
-                o.gemm_qkvg(uA, D, pk[f'qkvg{i}'], D, M, H, D, q, k, v, gates, qk_inv, self.P(f'{pre}.1.fn.q_norm.gamma'), self.P(f'{pre}.1.fn.k_norm.gamma'),
+                getattr(o, 'gemm_qkvg' + self.sfx)(uA, D, pk[f'qkvg{i}'], D, M, H, D, q, k, v, gates, qk_inv, self.P(f'{pre}.1.fn.q_norm.gamma'), self.P(f'{pre}.1.fn.k_norm.gamma'),
                             dv['rope_pos'], self.ws['rope_cs_t'], int(self.ws['rope_cs_t'].shape[1]), kv_rows, mixpre)
             else:
                 qk_inv = None
-                o.gemm_qkvg_rope(uA, D, pk[f'qkvg{i}'], D, M, H, D, q, k, v, gates, dv['rope_pos'], self.ws['rope_cs_t'], int(self.ws['rope_cs_t'].shape[1]),
-                                 kv_rows, mixpre)
+                getattr(o, 'gemm_qkvg_rope' + self.sfx)(uA, D, pk[f'qkvg{i}'], D, M, H, D, q, k, v, gates, dv['rope_pos'], self.ws['rope_cs_t'],
+                                                       int(self.ws['rope_cs_t'].shape[1]), kv_rows, mixpre)
             if has_mix:                                  # learned value residual (T.py:956-960): v = v mix + v_first_layer (1 - mix), in place (also on the cache rows)
                 v_first = cache.v[0] if cache is not None else st['layers'][0]['v']
-                o.vmix_fwd(v, HI, kv_rows, v_first, HI, mixpre, self.P(f'{pre}.1.fn.to_learned_value_residual.0.bias'), M, H)
+                getattr(o, 'vmix_fwd' + self.sfx)(v, HI, kv_rows, v_first, HI, mixpre, self.P(f'{pre}.1.fn.to_learned_value_residual.0.bias'), M, H)
             v_att, att_gates = v, gates
             if self.laser:                               # LASER (T.py:981-983): attention runs on exp(softclamp(v)); log + gate follow it
                 v_att = cache.vl[i] if cache is not None else self.buf(f'{lt}vl', (M, HI), BF16)
-                o.laser_v_fwd(v, HI, kv_rows, v_att, HI, M, H, self.laser_clamp)
+                o.laser_v_fwd(v, HI, kv_rows, v_att, HI, M, self.vheads, self.laser_clamp)
                 att_gates = None
             att = self.buf(f'{lt}o', (M, HI), BF16); lse = self.buf(f'{lt}lse', (H, M), F32)
             o_l = self.buf(f'{lt}ol', (M, HI), BF16) if self.laser else att
-            fp = self.fastp[i] if self.qk_norm else None
+            fp = self.fastp[i] if self.fast else None
             if getattr(rb, 'single_row_tiles', False):
                 # text decode: one query row per sample against its cache slab (split-KV decode kernel)
-                o.attn_decode(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['tile_q0'], dv['tile_kv0'], dv['tile_kvend'], n_tiles, o_l, HI, self.scale, self.softcap)
+                getattr(o, 'attn_decode' + self.sfx)(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['tile_q0'], dv['tile_kv0'], dv['tile_kvend'], n_tiles, o_l, HI, self.scale, self.softcap)
             else:
                 # both kernels are enqueued; the one whose precondition (read from `fp` on the device) fails returns immediately.  Without the
-                # qk-RMSNorm only the general kernel runs (fp = None)
-                if self.qk_norm:
+                # qk-RMSNorm, or at dim_head 128, only the general kernel runs (fp = None)
+                if self.fast:
                     o.attn_fwd_tc(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['t2_q0'], dv['t2_qend'], dv['t2_kv0'], dv['t2_kvend'], int(rb.t2_q0.shape[0]),
                                   o_l, HI, lse, M, M_kv, self.scale, self.softcap, fp)
-                o.attn_fwd(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['tile_q0'], dv['tile_qend'], dv['tile_kv0'], dv['tile_kvend'], n_tiles,
-                           o_l, HI, lse, M, self.scale, self.softcap, fp)
+                if self.d128:
+                    o.attn_fwd_d128(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['tile_q0'], dv['tile_qend'], dv['tile_kv0'], dv['tile_kvend'],
+                                    n_tiles, o_l, HI, lse, M, self.scale, self.softcap)
+                else:
+                    o.attn_fwd(q, k, v_att, HI, HI, HI, att_gates, H, dv['kv_limit'], dv['tile_q0'], dv['tile_qend'], dv['tile_kv0'], dv['tile_kvend'], n_tiles,
+                               o_l, HI, lse, M, self.scale, self.softcap, fp)
             if self.laser:
-                o.laser_out_fwd(o_l, gates, att, M, H)
+                getattr(o, 'laser_out_fwd' + self.sfx)(o_l, gates, att, M, H)
             x_b = self.buf(f'{lt}xb', (M, D), F32); yA = self.buf(f'{lt}yA', (M, D), BF16) if train else None
             o.gemm_resid(att, HI, None, 0, 0, pk[f'wo{i}'], HI, M, D, HI, None, x_a, x_b, None, yA, cond_row, zgA, zg_ld, self.P(f'{pre}.1.layerscale'))
             uF = self.buf(f'{lt}uF', (M, D), BF16); statsF = self.buf(f'{lt}sF', (M, 2), F32)
@@ -901,37 +921,41 @@ class Engine:
             dop = self.buf('dop', (M, HI), BF16); dsum_hm = self.buf('dsum_hm', (H, M), F32); dsum_mh = self.buf('dsum_mh', (M, H), F32)
             dq = self.buf('dq', (M, HI), F32); dk = self.buf('dk', (M, HI), F32)
             if self.laser:
-                o.laser_bwd_prep(dog, L['o_l'], L['gates'], dop, dsum_hm, dsum_mh, dq, M, H)
+                getattr(o, 'laser_bwd_prep' + self.sfx)(dog, L['o_l'], L['gates'], dop, dsum_hm, dsum_mh, dq, M, H)
             else:
-                o.attn_bwd_prep(dog, L['att'], L['gates'], dop, dsum_hm, dsum_mh, dq, M, H)
+                getattr(o, 'attn_bwd_prep' + self.sfx)(dog, L['att'], L['gates'], dop, dsum_hm, dsum_mh, dq, M, H)
             dqkvg = self.buf('dqkvg', (M, self.NQ), BF16)
             if i == self.depth - 1:
                 dqkvg[:, 3 * HI + H:].zero_()   # pad columns are never written by the kernels; cleared once per backward (inside captured graphs too)
-            fp = self.fastp[i] if self.qk_norm else None
-            if self.qk_norm:
+            fp = self.fastp[i] if self.fast else None
+            if self.fast:
                 o.attn_bwd_tc(L['q'], L['k'], L['v_att'], dop, HI, HI, HI, HI, L['lse'], dsum_hm, dv['kv_limit'], dv['k2_kv0'], dv['k2_kvend'], dv['k2_q0'], dv['k2_qend'],
                               dv['k2_order'], int(rb.k2_kv0.shape[0]), dq, dk, dqkvg[:, 2 * HI:], self.NQ, M, H, self.scale, self.softcap, fp)
-            o.attn_bwd(L['q'], L['k'], L['v_att'], dop, HI, HI, HI, HI, L['lse'], dsum_hm, dv['kv_limit'], dv['kt_kv0'], dv['kt_kvend'], dv['kt_q0'], dv['kt_qend'],
-                       int(rb.kt_kv0.shape[0]), dq, dk, dqkvg[:, 2 * HI:], self.NQ, M, H, self.scale, self.softcap, fp)
+            if self.d128:
+                o.attn_bwd_d128(L['q'], L['k'], L['v_att'], dop, HI, HI, HI, HI, L['lse'], dsum_hm, dv['kv_limit'], dv['kt_kv0'], dv['kt_kvend'], dv['kt_q0'],
+                                dv['kt_qend'], int(rb.kt_kv0.shape[0]), dq, dk, dqkvg[:, 2 * HI:], self.NQ, M, H, self.scale, self.softcap)
+            else:
+                o.attn_bwd(L['q'], L['k'], L['v_att'], dop, HI, HI, HI, HI, L['lse'], dsum_hm, dv['kv_limit'], dv['kt_kv0'], dv['kt_kvend'], dv['kt_q0'], dv['kt_qend'],
+                           int(rb.kt_kv0.shape[0]), dq, dk, dqkvg[:, 2 * HI:], self.NQ, M, H, self.scale, self.softcap, fp)
             dv_cols = dqkvg[:, 2 * HI:]
             if self.laser:                               # d v' -> d v (v' = exp(softclamp(v)))
-                o.laser_v_bwd(dv_cols, self.NQ, L['v'], HI, M, H, self.laser_clamp)
+                o.laser_v_bwd(dv_cols, self.NQ, L['v'], HI, M, self.vheads, self.laser_clamp)
             if self.vres:
                 dv0 = self.buf('dv_first', (M, HI), F32)
                 if i == self.depth - 1:
                     dv0.zero_()
                 if i > 0:                                # d v_mixed -> d v_raw; the first layer's share accumulates in dv0, d mix_pre goes to the packed column block
-                    o.vmix_bwd(dv_cols, self.NQ, L['v'], HI, st['layers'][0]['v'], HI, L['mixpre'], self.P(f'{pre}.1.fn.to_learned_value_residual.0.bias'), dv0,
-                               dqkvg[:, 3 * HI + H:], self.NQ, M, H)
-                    o.colsum_bf16(dqkvg[:, 3 * HI + H:], self.NQ, M, H, None, self.G(f'{pre}.1.fn.to_learned_value_residual.0.bias'))
+                    getattr(o, 'vmix_bwd' + self.sfx)(dv_cols, self.NQ, L['v'], HI, st['layers'][0]['v'], HI, L['mixpre'], self.P(f'{pre}.1.fn.to_learned_value_residual.0.bias'), dv0,
+                               dqkvg[:, self.MIX:], self.NQ, M, H)
+                    o.colsum_bf16(dqkvg[:, self.MIX:], self.NQ, M, H, None, self.G(f'{pre}.1.fn.to_learned_value_residual.0.bias'))
                 else:
-                    dqkvg[:, 3 * HI + H:3 * HI + 2 * H].zero_()      # the first layer has no mix Linear: its column block must not carry layer 1's values
+                    dqkvg[:, self.MIX:self.MIX + H].zero_()      # the first layer has no mix Linear: its column block must not carry layer 1's values
                     o.add_f32_into_bf16(dv_cols, self.NQ, dv0, HI, M, HI)
             if self.qk_norm:
-                o.qk_bwd_pack(dq, dk, L['q'], L['k'], L['qk_inv'], self.P(f'{pre}.1.fn.q_norm.gamma'), self.P(f'{pre}.1.fn.k_norm.gamma'), dv['rope_pos'],
+                getattr(o, 'qk_bwd_pack' + self.sfx)(dq, dk, L['q'], L['k'], L['qk_inv'], self.P(f'{pre}.1.fn.q_norm.gamma'), self.P(f'{pre}.1.fn.k_norm.gamma'), dv['rope_pos'],
                               self.ws['rope_cs'], L['gates'], dsum_mh, dqkvg, self.NQ, self.G(f'{pre}.1.fn.q_norm.gamma'), self.G(f'{pre}.1.fn.k_norm.gamma'), M, H)
             else:
-                o.qk_bwd_pack_rope(dq, dk, dv['rope_pos'], self.ws['rope_cs'], L['gates'], dsum_mh, dqkvg, self.NQ, M, H)
+                getattr(o, 'qk_bwd_pack_rope' + self.sfx)(dq, dk, dv['rope_pos'], self.ws['rope_cs'], L['gates'], dsum_mh, dqkvg, self.NQ, M, H)
             o.gemm_store(dqkvg, self.NQ, 0, pk[f'qkvg{i}'], D, 1, M, D, self.NQ, du, D, None, 0, None, None, 1.0, 0, 1)
             o.gemm_store(dqkvg, self.NQ, 1, L['uA'], D, 1, self.NQ, D, M, self.gflat, 0, None, 0, None, lm['qkvg_rows'], 1.0, 1, ksplit(self.NQ, D))
             o.adaln_bwd(du, L['x_a'], L['statsA'], cond_row, st['tab'][:, wA * 3 * D:] if nc > 0 else None, tab_ld, self.P(f'{pre}.1.layernorm_gamma'), gx,

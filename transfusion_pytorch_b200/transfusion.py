@@ -7,7 +7,7 @@ versa.  What differs is everything underneath: the modules below only OWN parame
 the block stack, attention, loss heads and optimizer runs in the sm_90a kernels of `libtfx_b200.so`
 driven by `engine.Engine` over the ragged descriptor of `modality_processing.pack_batch`.
 
-Out of scope here (raise loudly): U-Net pre/post encoders (`pre_post_transformer_enc_dec`), attention dropout, dim_head != 64, a custom
+Out of scope here (raise loudly): U-Net pre/post encoders (`pre_post_transformer_enc_dec`), attention dropout, dim_head other than 64 or 128, a custom
 `loss_fn` of `SelfMaskedRepTraining`.  `qk_rmsnorm = False` is supported: the q / k norm gammas are still built (same state-dict keys) and get
 no gradient, as in the reference.
 """
@@ -34,6 +34,8 @@ MAX_DEPTH = 64
 MODEL_DIMS = (128, 256, 384, 512, 768, 1024)
 # Heads the attention kernels take: two 64-wide heads per 128-column GEMM tile, at most 32 (gemm_qkvg's 32-column gate slab)
 MIN_HEADS, MAX_HEADS = 2, 32
+DIM_HEADS = (64, 128)                # attention head widths the kernels implement
+MAX_HEADS_D128 = 16                  # heads at dim_head = 128 (inner width <= 2048, as at 64)
 
 
 class TextKVCache:
@@ -211,10 +213,12 @@ class Transformer(Module):
                  use_value_residual = False):
         super().__init__()
         unsupported = []
-        if dim_head != 64: unsupported.append('dim_head != 64')
+        if dim_head not in DIM_HEADS: unsupported.append(f'dim_head {dim_head} (the attention kernels take {" or ".join(map(str, DIM_HEADS))})')
         if depth > MAX_DEPTH: unsupported.append(f'depth {depth} > {MAX_DEPTH}')
         if dim not in MODEL_DIMS: unsupported.append(f'dim {dim} (the row kernels take {", ".join(map(str, MODEL_DIMS))})')
-        if heads % 2 or not MIN_HEADS <= heads <= MAX_HEADS: unsupported.append(f'heads {heads} (must be even and in [{MIN_HEADS}, {MAX_HEADS}])')
+        if dim_head == 128:                          # one head fills a 128-column QKVG tile: any count up to the 2048-wide inner limit
+            if not 1 <= heads <= MAX_HEADS_D128: unsupported.append(f'heads {heads} at dim_head 128 (must be in [1, {MAX_HEADS_D128}])')
+        elif heads % 2 or not MIN_HEADS <= heads <= MAX_HEADS: unsupported.append(f'heads {heads} (must be even and in [{MIN_HEADS}, {MAX_HEADS}])')
         ff_dropout = float(ff_kwargs.get('dropout', 0.))
         for name, p in (('dropout', dropout), ("ff_kwargs['dropout']", ff_dropout)):
             if not 0. <= p <= 1.:
