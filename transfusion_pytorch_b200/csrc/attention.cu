@@ -6,8 +6,9 @@
 // o = softmax_j(s) v ;  o *= sigmoid(gate[i, head]).
 // The mask is evaluated from one int per query row in registers - no N x N mask or score tensor exists.
 //
-// Layout: token-major q/k/v/o [M_total][heads*64] bf16, sequences packed back to back; 64-row tiles
-// never straddle a sequence (host builds the tile tables).
+// Layout: token-major q/k/v/o [M_total][heads*DH] bf16 (head dim DH = 64 or 128), sequences packed back to back; 64-row tiles
+// never straddle a sequence (host builds the tile tables).  The forward and the backward pre-pass are templates on DH; the backward main
+// pass is attn_bwd_k at 64 and attn_bwd_dh_k (8 warps) at 128.
 // Math: bf16 mma.sync m16n8k16 with fp32 accumulation, online softmax in registers (FlashAttention-2
 // schedule).  The score path is MUFU-bound (tanh + exp per score), not tensor-bound, at head dim 64.
 #include "common.cuh"
@@ -15,11 +16,11 @@
 
 namespace tfx {
 
-constexpr int ATT_BM = 64, ATT_BN = 64, ATT_DH = 64, ATT_THREADS = 128;
+constexpr int ATT_BM = 64, ATT_BN = 64, ATT_THREADS = 128;
 constexpr int ATT_BWD_SMEM = 7 * 64 * 64 * 2 + 6 * 64 * 4;
-// head dim 128 (attn_fwd_dh_k / attn_bwd_dh_k below): Q and the K / V double buffers; K, V, double-buffered Q / dO, dS^T, the dS weights
-// of the four key groups and the per-query rows
-constexpr int ATT_FWD_SMEM_D128 = 5 * 64 * 128 * 2;
+// attn_fwd_k: Q and the K / V double buffers
+constexpr int att_fwd_smem(int dh) { return 5 * 64 * dh * 2; }
+// head dim 128 (attn_bwd_dh_k below): K, V, double-buffered Q / dO, dS^T, the dS weights of the four key groups and the per-query rows
 constexpr int ATT_BWD_THREADS_D128 = 256;
 constexpr int ATT_BWD_SMEM_D128 = 6 * 64 * 128 * 2 + 64 * 64 * 2 + 4 * 16 * 64 * 4 + 6 * 64 * 4;
 
@@ -43,11 +44,11 @@ __device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], 
 }
 
 // tile element (row, 16-byte chunk) -> swizzled bf16 offset inside a [64][DH] tile (the xor stays inside each group of 8 chunks)
-template <int DH = 64>
+template <int DH>
 __device__ __forceinline__ int swz(int row, int chunk) { return row * DH + ((chunk ^ (row & 7)) << 3); }
 
 // cooperative async load of a [64 rows][DH bf16] tile by NT threads; rows >= row_end are zero filled
-template <int DH = 64, int NT = ATT_THREADS>
+template <int DH, int NT = ATT_THREADS>
 __device__ __forceinline__ void load_tile(__nv_bfloat16* s, const __nv_bfloat16* g, long long ld, int row0, int row_end, int tid) {
   constexpr int SH = DH == 64 ? 3 : 4;       // log2 of the 16-byte chunks per row
 #pragma unroll
@@ -67,27 +68,43 @@ __device__ __forceinline__ float tanh_acc(float x) {
 }
 
 // ================================================================================================ forward
+// One CTA per (64-query tile, head), 4 warps of 16 query rows; K / V tiles double-buffered through cp.async.  The whole head is held in
+// registers (oacc DH / 2, qf DH / 4 per thread).
+template <int DH>
 __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_k(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k, const __nv_bfloat16* __restrict__ v,
                                                          long long ld_q, long long ld_k, long long ld_v, const float* __restrict__ gates, int H,
                                                          const int* __restrict__ kv_limit, const int* __restrict__ tile_q0, const int* __restrict__ tile_qend,
                                                          const int* __restrict__ tile_kv0, const int* __restrict__ tile_kvend, __nv_bfloat16* __restrict__ o,
                                                          long long ld_o, float* __restrict__ lse, int M, float scale, float cap, const float* __restrict__ skip_if_fast) {
-  if (skip_if_fast && skip_if_fast[0] != 0.f) return;     // the bounded-logit wgmma kernel (attention_sm90.cu) handles this layer
-  __shared__ __align__(128) __nv_bfloat16 sQ[64 * 64];
-  __shared__ __align__(128) __nv_bfloat16 sK[2][64 * 64];
-  __shared__ __align__(128) __nv_bfloat16 sV[2][64 * 64];
+  // the bounded-logit wgmma kernel (attention_sm90.cu, head dim 64 only) handles this layer
+  if (DH == 64 && skip_if_fast && skip_if_fast[0] != 0.f) return;
+  constexpr int TILE = 64 * DH;
+  __nv_bfloat16* sQ;
+  __nv_bfloat16 (*sK)[TILE];     // [2][TILE]
+  __nv_bfloat16 (*sV)[TILE];     // [2][TILE]
+  if constexpr (DH == 64) {          // 40 KB fit in static shared memory; the 80 KB of DH = 128 need the dynamic opt-in
+    __shared__ __align__(128) __nv_bfloat16 sQs[TILE];
+    __shared__ __align__(128) __nv_bfloat16 sKs[2][TILE];
+    __shared__ __align__(128) __nv_bfloat16 sVs[2][TILE];
+    sQ = sQs; sK = sKs; sV = sVs;
+  } else {
+    extern __shared__ __align__(128) uint8_t att_smem[];
+    sQ = reinterpret_cast<__nv_bfloat16*>(att_smem);
+    sK = reinterpret_cast<__nv_bfloat16 (*)[TILE]>(sQ + TILE);
+    sV = reinterpret_cast<__nv_bfloat16 (*)[TILE]>(sQ + 3 * TILE);
+  }
   const int tile = gridDim.x - 1 - blockIdx.x;      // heavy (late) tiles first
   const int head = blockIdx.y;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
   const int q0 = tile_q0[tile], q_end = tile_qend[tile], kv0 = tile_kv0[tile], kv_end = tile_kvend[tile];
-  const __nv_bfloat16* qh = q + head * 64;
-  const __nv_bfloat16* kh = k + head * 64;
-  const __nv_bfloat16* vh = v + head * 64;
+  const __nv_bfloat16* qh = q + head * DH;
+  const __nv_bfloat16* kh = k + head * DH;
+  const __nv_bfloat16* vh = v + head * DH;
 
-  load_tile(sQ, qh, ld_q, q0, q_end, tid);
+  load_tile<DH>(sQ, qh, ld_q, q0, q_end, tid);
   const int n_kv = (kv_end - kv0 + ATT_BN - 1) / ATT_BN;
-  load_tile(sK[0], kh, ld_k, kv0, kv_end, tid);
-  load_tile(sV[0], vh, ld_v, kv0, kv_end, tid);
+  load_tile<DH>(sK[0], kh, ld_k, kv0, kv_end, tid);
+  load_tile<DH>(sV[0], vh, ld_v, kv0, kv_end, tid);
   cp_async_commit();
 
   const int row_a = q0 + warp * 16 + g, row_b = row_a + 8;
@@ -98,19 +115,19 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_k(const __nv_bfloat16* _
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) wlim = max(wlim, __shfl_xor_sync(0xffffffffu, wlim, off));
 
-  float oacc[8][4];
+  float oacc[DH / 8][4];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) { oacc[i][0] = oacc[i][1] = oacc[i][2] = oacc[i][3] = 0.f; }
+  for (int i = 0; i < DH / 8; ++i) { oacc[i][0] = oacc[i][1] = oacc[i][2] = oacc[i][3] = 0.f; }
   float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f;
-  uint32_t qf[4][4];
+  uint32_t qf[DH / 16][4];
   const float inv_cap = 1.f / cap;
   const float LOG2E = 1.4426950408889634f;
 
   for (int j = 0; j < n_kv; ++j) {
     const int buf = j & 1;
     if (j + 1 < n_kv) {
-      load_tile(sK[buf ^ 1], kh, ld_k, kv0 + (j + 1) * ATT_BN, kv_end, tid);
-      load_tile(sV[buf ^ 1], vh, ld_v, kv0 + (j + 1) * ATT_BN, kv_end, tid);
+      load_tile<DH>(sK[buf ^ 1], kh, ld_k, kv0 + (j + 1) * ATT_BN, kv_end, tid);
+      load_tile<DH>(sV[buf ^ 1], vh, ld_v, kv0 + (j + 1) * ATT_BN, kv_end, tid);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -119,10 +136,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_k(const __nv_bfloat16* _
     __syncthreads();
     if (j == 0) {
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
+      for (int ks = 0; ks < DH / 16; ++ks) {
         const int mat = lane >> 3;
         const int row = warp * 16 + (mat & 1) * 8 + (lane & 7);
-        ldsm_x4(s_u32(sQ + swz(row, ks * 2 + (mat >> 1))), qf[ks][0], qf[ks][1], qf[ks][2], qf[ks][3]);
+        ldsm_x4(s_u32(sQ + swz<DH>(row, ks * 2 + (mat >> 1))), qf[ks][0], qf[ks][1], qf[ks][2], qf[ks][3]);
       }
     }
     const int key0 = kv0 + j * ATT_BN;
@@ -132,13 +149,13 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_k(const __nv_bfloat16* _
 #pragma unroll
       for (int i = 0; i < 8; ++i) { sacc[i][0] = sacc[i][1] = sacc[i][2] = sacc[i][3] = 0.f; }
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
+      for (int ks = 0; ks < DH / 16; ++ks) {
 #pragma unroll
         for (int np = 0; np < 4; ++np) {
           const int mat = lane >> 3;
           const int row = np * 16 + (mat >> 1) * 8 + (lane & 7);
           uint32_t b0, b1, b2, b3;
-          ldsm_x4(s_u32(sK[buf] + swz(row, ks * 2 + (mat & 1))), b0, b1, b2, b3);
+          ldsm_x4(s_u32(sK[buf] + swz<DH>(row, ks * 2 + (mat & 1))), b0, b1, b2, b3);
           mma_bf16(sacc[2 * np], qf[ks], b0, b1);
           mma_bf16(sacc[2 * np + 1], qf[ks], b2, b3);
         }
@@ -174,16 +191,16 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_k(const __nv_bfloat16* _
       }
       l_a = l_a * ca + ra; l_b = l_b * cb + rb;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) { oacc[i][0] *= ca; oacc[i][1] *= ca; oacc[i][2] *= cb; oacc[i][3] *= cb; }
+      for (int i = 0; i < DH / 8; ++i) { oacc[i][0] *= ca; oacc[i][1] *= ca; oacc[i][2] *= cb; oacc[i][3] *= cb; }
       // ---- O += P V
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {
 #pragma unroll
-        for (int dp = 0; dp < 4; ++dp) {
+        for (int dp = 0; dp < DH / 16; ++dp) {
           const int mat = lane >> 3;
           const int row = kk * 16 + (mat & 1) * 8 + (lane & 7);
           uint32_t b0, b1, b2, b3;
-          ldsm_x4_t(s_u32(sV[buf] + swz(row, dp * 2 + (mat >> 1))), b0, b1, b2, b3);
+          ldsm_x4_t(s_u32(sV[buf] + swz<DH>(row, dp * 2 + (mat >> 1))), b0, b1, b2, b3);
           mma_bf16(oacc[2 * dp], pf[kk], b0, b1);
           mma_bf16(oacc[2 * dp + 1], pf[kk], b2, b3);
         }
@@ -201,32 +218,36 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_k(const __nv_bfloat16* _
     if (row_b < q_end) gb = 1.f / (1.f + __expf(-gates[(long long)row_b * H + head]));
   }
   if (row_a < q_end) {
-    __nv_bfloat16* dst = o + (long long)row_a * ld_o + head * 64 + 2 * t;
+    __nv_bfloat16* dst = o + (long long)row_a * ld_o + head * DH + 2 * t;
 #pragma unroll
-    for (int nt = 0; nt < 8; ++nt) *reinterpret_cast<uint32_t*>(dst + nt * 8) = pack2_bf16(oacc[nt][0] * ia * ga, oacc[nt][1] * ia * ga);
+    for (int nt = 0; nt < DH / 8; ++nt) *reinterpret_cast<uint32_t*>(dst + nt * 8) = pack2_bf16(oacc[nt][0] * ia * ga, oacc[nt][1] * ia * ga);
     if (t == 0 && lse) lse[(long long)head * M + row_a] = m_a + logf(l_a);
   }
   if (row_b < q_end) {
-    __nv_bfloat16* dst = o + (long long)row_b * ld_o + head * 64 + 2 * t;
+    __nv_bfloat16* dst = o + (long long)row_b * ld_o + head * DH + 2 * t;
 #pragma unroll
-    for (int nt = 0; nt < 8; ++nt) *reinterpret_cast<uint32_t*>(dst + nt * 8) = pack2_bf16(oacc[nt][2] * ib * gb, oacc[nt][3] * ib * gb);
+    for (int nt = 0; nt < DH / 8; ++nt) *reinterpret_cast<uint32_t*>(dst + nt * 8) = pack2_bf16(oacc[nt][2] * ib * gb, oacc[nt][3] * ib * gb);
     if (t == 0 && lse) lse[(long long)head * M + row_b] = m_b + logf(l_b);
   }
 }
 
 // ================================================================================================ backward
 // pre-pass (one warp per token): dsum[h][row] = sum_d dO_gated*O_gated ; dO_pre = dO_gated * sigmoid(gate) ; dq accumulator cleared.
-// 8 lanes share a head (16-byte bf16 accesses), 4 heads per pass, the per-head dot product is a 3-step shuffle.
+// DH / 8 lanes share a head (16-byte bf16 accesses; 8 at DH = 64, 16 at 128), 32 / (DH / 8) heads per pass, the per-head dot product is a
+// log2(DH / 8)-step shuffle.
+template <int DH>
 __global__ void __launch_bounds__(ROW_THREADS) attn_bwd_prep_k(const __nv_bfloat16* __restrict__ dog, const __nv_bfloat16* __restrict__ og, const float* __restrict__ gates,
-                                                              __nv_bfloat16* __restrict__ dop, float* __restrict__ dsum, float* __restrict__ dsum_rowmajor, float* __restrict__ dq_zero, int M, int H) {
-  const int lane = threadIdx.x & 31, sub = lane & 7, hq = lane >> 3;
+                                                              __nv_bfloat16* __restrict__ dop, float* __restrict__ dsum, float* __restrict__ dsum_rowmajor,
+                                                              float* __restrict__ dq_zero, int M, int H) {
+  constexpr int LPH = DH / 8, HPP = 32 / LPH;
+  const int lane = threadIdx.x & 31, sub = lane % LPH, hq = (lane >> 3) / (LPH / 8);
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-  const int HI = H * 64;
+  const int HI = H * DH;
   for (int row = warp0; row < M; row += nwarps) {
-    for (int h0 = 0; h0 < H; h0 += 4) {
+    for (int h0 = 0; h0 < H; h0 += HPP) {
       const int h = h0 + hq;
       const bool act = h < H;
-      const long long off = (long long)row * HI + (act ? h : 0) * 64 + sub * 8;
+      const long long off = (long long)row * HI + (act ? h : 0) * DH + sub * 8;
       const uint4 a4 = *reinterpret_cast<const uint4*>(dog + off), b4 = *reinterpret_cast<const uint4*>(og + off);
       const float sg = (act && gates) ? 1.f / (1.f + __expf(-gates[(long long)row * H + h])) : 1.f;
       const uint32_t aw[4] = {a4.x, a4.y, a4.z, a4.w}, bw[4] = {b4.x, b4.y, b4.z, b4.w};
@@ -238,7 +259,8 @@ __global__ void __launch_bounds__(ROW_THREADS) attn_bwd_prep_k(const __nv_bfloat
         s += a.x * b.x + a.y * b.y;
         ow[e] = pack2_bf16(a.x * sg, a.y * sg);
       }
-      s += __shfl_xor_sync(0xffffffffu, s, 1); s += __shfl_xor_sync(0xffffffffu, s, 2); s += __shfl_xor_sync(0xffffffffu, s, 4);
+#pragma unroll
+      for (int o = 1; o < LPH; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
       if (act) {
         *reinterpret_cast<uint4*>(dop + off) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
         if (sub == 0) { dsum[(long long)h * M + row] = s; if (dsum_rowmajor) dsum_rowmajor[(long long)row * H + h] = s; }
@@ -287,8 +309,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_k(const __nv_bfloat16* _
 
   auto load_q = [&](int buf, int i) {
     const int r0 = q_begin + i * 64;
-    load_tile(sQ_(buf), qh, ld_q, r0, q_end, tid);
-    load_tile(sDO_(buf), doh, ld_do, r0, q_end, tid);
+    load_tile<64>(sQ_(buf), qh, ld_q, r0, q_end, tid);
+    load_tile<64>(sDO_(buf), doh, ld_do, r0, q_end, tid);
     if (tid < 64) {
       const int r = r0 + tid;
       const bool ok = r < q_end;
@@ -297,8 +319,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_k(const __nv_bfloat16* _
       sLim_(buf)[tid] = ok ? kv_limit[r] : -1;
     }
   };
-  load_tile(sK, k + head * 64, ld_k, kv0, kv_end, tid);
-  load_tile(sV, v + head * 64, ld_v, kv0, kv_end, tid);
+  load_tile<64>(sK, k + head * 64, ld_k, kv0, kv_end, tid);
+  load_tile<64>(sV, v + head * 64, ld_v, kv0, kv_end, tid);
   if (n_q > 0) load_q(0, 0);
   cp_async_commit();
 
@@ -322,18 +344,18 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_k(const __nv_bfloat16* _
       {
         const int mat = lane >> 3;
         const int row = warp * 16 + (mat & 1) * 8 + (lane & 7);
-        ldsm_x4(s_u32(sK + swz(row, ks * 2 + (mat >> 1))), ka[0], ka[1], ka[2], ka[3]);
-        ldsm_x4(s_u32(sV + swz(row, ks * 2 + (mat >> 1))), va[0], va[1], va[2], va[3]);
+        ldsm_x4(s_u32(sK + swz<64>(row, ks * 2 + (mat >> 1))), ka[0], ka[1], ka[2], ka[3]);
+        ldsm_x4(s_u32(sV + swz<64>(row, ks * 2 + (mat >> 1))), va[0], va[1], va[2], va[3]);
       }
 #pragma unroll
       for (int np = 0; np < 4; ++np) {
         const int mat = lane >> 3;
         const int row = np * 16 + (mat >> 1) * 8 + (lane & 7);
         uint32_t b0, b1, b2, b3;
-        ldsm_x4(s_u32(sQ_(buf) + swz(row, ks * 2 + (mat & 1))), b0, b1, b2, b3);
+        ldsm_x4(s_u32(sQ_(buf) + swz<64>(row, ks * 2 + (mat & 1))), b0, b1, b2, b3);
         mma_bf16(sacc[2 * np], ka, b0, b1);
         mma_bf16(sacc[2 * np + 1], ka, b2, b3);
-        ldsm_x4(s_u32(sDO_(buf) + swz(row, ks * 2 + (mat & 1))), b0, b1, b2, b3);
+        ldsm_x4(s_u32(sDO_(buf) + swz<64>(row, ks * 2 + (mat & 1))), b0, b1, b2, b3);
         mma_bf16(pacc[2 * np], va, b0, b1);
         mma_bf16(pacc[2 * np + 1], va, b2, b3);
       }
@@ -359,8 +381,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_k(const __nv_bfloat16* _
       dsf[nt >> 1][(nt & 1) * 2 + 1] = pack2_bf16(dv_[2], dv_[3]);
       // stage dS^T [key][query] for the dQ product
       const int ch = nt;   // 8 queries per chunk
-      *reinterpret_cast<uint32_t*>(sDS + swz(warp * 16 + g, ch) + 2 * t) = dsf[nt >> 1][(nt & 1) * 2];
-      *reinterpret_cast<uint32_t*>(sDS + swz(warp * 16 + g + 8, ch) + 2 * t) = dsf[nt >> 1][(nt & 1) * 2 + 1];
+      *reinterpret_cast<uint32_t*>(sDS + swz<64>(warp * 16 + g, ch) + 2 * t) = dsf[nt >> 1][(nt & 1) * 2];
+      *reinterpret_cast<uint32_t*>(sDS + swz<64>(warp * 16 + g + 8, ch) + 2 * t) = dsf[nt >> 1][(nt & 1) * 2 + 1];
     }
     // ---- dV += P^T dO ;  dK += dS^T Q       (k-dim = queries, B row-major [query][d] -> transposed ldmatrix)
 #pragma unroll
@@ -370,10 +392,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_k(const __nv_bfloat16* _
         const int mat = lane >> 3;
         const int row = kk * 16 + (mat & 1) * 8 + (lane & 7);
         uint32_t b0, b1, b2, b3;
-        ldsm_x4_t(s_u32(sDO_(buf) + swz(row, dp * 2 + (mat >> 1))), b0, b1, b2, b3);
+        ldsm_x4_t(s_u32(sDO_(buf) + swz<64>(row, dp * 2 + (mat >> 1))), b0, b1, b2, b3);
         mma_bf16(dvacc[2 * dp], pf[kk], b0, b1);
         mma_bf16(dvacc[2 * dp + 1], pf[kk], b2, b3);
-        ldsm_x4_t(s_u32(sQ_(buf) + swz(row, dp * 2 + (mat >> 1))), b0, b1, b2, b3);
+        ldsm_x4_t(s_u32(sQ_(buf) + swz<64>(row, dp * 2 + (mat >> 1))), b0, b1, b2, b3);
         mma_bf16(dkacc[2 * dp], dsf[kk], b0, b1);
         mma_bf16(dkacc[2 * dp + 1], dsf[kk], b2, b3);
       }
@@ -393,14 +415,14 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_k(const __nv_bfloat16* _
           const int mat = lane >> 3;
           const int krow = kk * 16 + (mat >> 1) * 8 + (lane & 7);
           const int qchunk = warp * 2 + (mat & 1);
-          ldsm_x4_t(s_u32(sDS + swz(krow, qchunk)), a[0], a[1], a[2], a[3]);
+          ldsm_x4_t(s_u32(sDS + swz<64>(krow, qchunk)), a[0], a[1], a[2], a[3]);
         }
 #pragma unroll
         for (int dp = 0; dp < 4; ++dp) {
           const int mat = lane >> 3;
           const int row = kk * 16 + (mat & 1) * 8 + (lane & 7);
           uint32_t b0, b1, b2, b3;
-          ldsm_x4_t(s_u32(sK + swz(row, dp * 2 + (mat >> 1))), b0, b1, b2, b3);
+          ldsm_x4_t(s_u32(sK + swz<64>(row, dp * 2 + (mat >> 1))), b0, b1, b2, b3);
           mma_bf16(qacc[2 * dp], a, b0, b1);
           mma_bf16(qacc[2 * dp + 1], a, b2, b3);
         }
@@ -434,198 +456,8 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_k(const __nv_bfloat16* _
   }
 }
 
-// ================================================================================================ head dim 128
-// The kernels above are the head-dim-64 ones.  These take the head dim as a template parameter and are instantiated at 128 only: the
-// 64-wide kernels keep their own code, because inlining them from a shared template body changes their generated code.
-// Same tile tables, span mask, soft-cap and gate.
-
-// forward: the 64-wide schedule with the whole 128-wide head in registers (oacc 64, qf 32 per thread); Q / K / V tiles in dynamic smem
-template <int DH>
-__global__ void __launch_bounds__(ATT_THREADS) attn_fwd_dh_k(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k, const __nv_bfloat16* __restrict__ v,
-                                                            long long ld_q, long long ld_k, long long ld_v, const float* __restrict__ gates, int H,
-                                                            const int* __restrict__ kv_limit, const int* __restrict__ tile_q0, const int* __restrict__ tile_qend,
-                                                            const int* __restrict__ tile_kv0, const int* __restrict__ tile_kvend, __nv_bfloat16* __restrict__ o,
-                                                            long long ld_o, float* __restrict__ lse, int M, float scale, float cap) {
-  constexpr int TILE = 64 * DH;
-  extern __shared__ __align__(128) uint8_t att_smem[];
-  __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(att_smem);
-  __nv_bfloat16* sK = sQ + TILE;          // [2][TILE]
-  __nv_bfloat16* sV = sQ + 3 * TILE;      // [2][TILE]
-  const int tile = gridDim.x - 1 - blockIdx.x;      // heavy (late) tiles first
-  const int head = blockIdx.y;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
-  const int q0 = tile_q0[tile], q_end = tile_qend[tile], kv0 = tile_kv0[tile], kv_end = tile_kvend[tile];
-  const __nv_bfloat16* qh = q + head * DH;
-  const __nv_bfloat16* kh = k + head * DH;
-  const __nv_bfloat16* vh = v + head * DH;
-
-  load_tile<DH>(sQ, qh, ld_q, q0, q_end, tid);
-  const int n_kv = (kv_end - kv0 + ATT_BN - 1) / ATT_BN;
-  load_tile<DH>(sK, kh, ld_k, kv0, kv_end, tid);
-  load_tile<DH>(sV, vh, ld_v, kv0, kv_end, tid);
-  cp_async_commit();
-
-  const int row_a = q0 + warp * 16 + g, row_b = row_a + 8;
-  const int lim_a = row_a < q_end ? kv_limit[row_a] : -1;
-  const int lim_b = row_b < q_end ? kv_limit[row_b] : -1;
-  int wlim = max(lim_a, lim_b);
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) wlim = max(wlim, __shfl_xor_sync(0xffffffffu, wlim, off));
-
-  float oacc[DH / 8][4];
-#pragma unroll
-  for (int i = 0; i < DH / 8; ++i) { oacc[i][0] = oacc[i][1] = oacc[i][2] = oacc[i][3] = 0.f; }
-  float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f;
-  uint32_t qf[DH / 16][4];
-  const float inv_cap = 1.f / cap;
-  const float LOG2E = 1.4426950408889634f;
-
-  for (int j = 0; j < n_kv; ++j) {
-    const int buf = j & 1;
-    if (j + 1 < n_kv) {
-      load_tile<DH>(sK + (buf ^ 1) * TILE, kh, ld_k, kv0 + (j + 1) * ATT_BN, kv_end, tid);
-      load_tile<DH>(sV + (buf ^ 1) * TILE, vh, ld_v, kv0 + (j + 1) * ATT_BN, kv_end, tid);
-      cp_async_commit();
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
-    __syncthreads();
-    if (j == 0) {
-#pragma unroll
-      for (int ks = 0; ks < DH / 16; ++ks) {
-        const int mat = lane >> 3;
-        const int row = warp * 16 + (mat & 1) * 8 + (lane & 7);
-        ldsm_x4(s_u32(sQ + swz<DH>(row, ks * 2 + (mat >> 1))), qf[ks][0], qf[ks][1], qf[ks][2], qf[ks][3]);
-      }
-    }
-    const int key0 = kv0 + j * ATT_BN;
-    if (key0 <= wlim) {
-      // ---- S = Q K^T
-      float sacc[8][4];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) { sacc[i][0] = sacc[i][1] = sacc[i][2] = sacc[i][3] = 0.f; }
-#pragma unroll
-      for (int ks = 0; ks < DH / 16; ++ks) {
-#pragma unroll
-        for (int np = 0; np < 4; ++np) {
-          const int mat = lane >> 3;
-          const int row = np * 16 + (mat >> 1) * 8 + (lane & 7);
-          uint32_t b0, b1, b2, b3;
-          ldsm_x4(s_u32(sK + buf * TILE + swz<DH>(row, ks * 2 + (mat & 1))), b0, b1, b2, b3);
-          mma_bf16(sacc[2 * np], qf[ks], b0, b1);
-          mma_bf16(sacc[2 * np + 1], qf[ks], b2, b3);
-        }
-      }
-      // ---- soft-cap, mask, online softmax
-      float mx_a = m_a, mx_b = m_b;
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int key = key0 + nt * 8 + 2 * t + (e & 1);
-          const int lim = (e < 2) ? lim_a : lim_b;
-          float s = cap * tanh_acc(sacc[nt][e] * scale * inv_cap);
-          s = key <= lim ? s : -INFINITY;
-          sacc[nt][e] = s;
-          if (e < 2) mx_a = fmaxf(mx_a, s); else mx_b = fmaxf(mx_b, s);
-        }
-      }
-      mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1)); mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
-      mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1)); mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
-      const float ma_s = mx_a == -INFINITY ? 0.f : mx_a, mb_s = mx_b == -INFINITY ? 0.f : mx_b;   // fully masked rows stay at p = 0
-      const float ca = exp2f((m_a - ma_s) * LOG2E), cb = exp2f((m_b - mb_s) * LOG2E);
-      m_a = mx_a; m_b = mx_b;
-      float ra = 0.f, rb = 0.f;
-      uint32_t pf[4][4];
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-        const float p0 = exp2f((sacc[nt][0] - ma_s) * LOG2E), p1 = exp2f((sacc[nt][1] - ma_s) * LOG2E);
-        const float p2 = exp2f((sacc[nt][2] - mb_s) * LOG2E), p3 = exp2f((sacc[nt][3] - mb_s) * LOG2E);
-        ra += p0 + p1; rb += p2 + p3;
-        pf[nt >> 1][(nt & 1) * 2] = pack2_bf16(p0, p1);
-        pf[nt >> 1][(nt & 1) * 2 + 1] = pack2_bf16(p2, p3);
-      }
-      l_a = l_a * ca + ra; l_b = l_b * cb + rb;
-#pragma unroll
-      for (int i = 0; i < DH / 8; ++i) { oacc[i][0] *= ca; oacc[i][1] *= ca; oacc[i][2] *= cb; oacc[i][3] *= cb; }
-      // ---- O += P V
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-        for (int dp = 0; dp < DH / 16; ++dp) {
-          const int mat = lane >> 3;
-          const int row = kk * 16 + (mat & 1) * 8 + (lane & 7);
-          uint32_t b0, b1, b2, b3;
-          ldsm_x4_t(s_u32(sV + buf * TILE + swz<DH>(row, dp * 2 + (mat >> 1))), b0, b1, b2, b3);
-          mma_bf16(oacc[2 * dp], pf[kk], b0, b1);
-          mma_bf16(oacc[2 * dp + 1], pf[kk], b2, b3);
-        }
-      }
-    }
-    __syncthreads();
-  }
-  // ---- epilogue: normalise, value gate, store
-  l_a += __shfl_xor_sync(0xffffffffu, l_a, 1); l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
-  l_b += __shfl_xor_sync(0xffffffffu, l_b, 1); l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
-  const float ia = l_a > 0.f ? 1.f / l_a : 0.f, ib = l_b > 0.f ? 1.f / l_b : 0.f;
-  float ga = 1.f, gb = 1.f;
-  if (gates) {
-    if (row_a < q_end) ga = 1.f / (1.f + __expf(-gates[(long long)row_a * H + head]));
-    if (row_b < q_end) gb = 1.f / (1.f + __expf(-gates[(long long)row_b * H + head]));
-  }
-  if (row_a < q_end) {
-    __nv_bfloat16* dst = o + (long long)row_a * ld_o + head * DH + 2 * t;
-#pragma unroll
-    for (int nt = 0; nt < DH / 8; ++nt) *reinterpret_cast<uint32_t*>(dst + nt * 8) = pack2_bf16(oacc[nt][0] * ia * ga, oacc[nt][1] * ia * ga);
-    if (t == 0 && lse) lse[(long long)head * M + row_a] = m_a + logf(l_a);
-  }
-  if (row_b < q_end) {
-    __nv_bfloat16* dst = o + (long long)row_b * ld_o + head * DH + 2 * t;
-#pragma unroll
-    for (int nt = 0; nt < DH / 8; ++nt) *reinterpret_cast<uint32_t*>(dst + nt * 8) = pack2_bf16(oacc[nt][2] * ib * gb, oacc[nt][3] * ib * gb);
-    if (t == 0 && lse) lse[(long long)head * M + row_b] = m_b + logf(l_b);
-  }
-}
-
-// backward pre-pass: attn_bwd_prep_k with DH / 8 lanes per head (16 at DH = 128), 32 / (DH / 8) heads per pass
-template <int DH>
-__global__ void __launch_bounds__(ROW_THREADS) attn_bwd_prep_dh_k(const __nv_bfloat16* __restrict__ dog, const __nv_bfloat16* __restrict__ og, const float* __restrict__ gates,
-                                                                 __nv_bfloat16* __restrict__ dop, float* __restrict__ dsum, float* __restrict__ dsum_rowmajor,
-                                                                 float* __restrict__ dq_zero, int M, int H) {
-  constexpr int LPH = DH / 8, HPP = 32 / LPH;
-  const int lane = threadIdx.x & 31, sub = lane % LPH, hq = lane / LPH;
-  const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-  const int HI = H * DH;
-  for (int row = warp0; row < M; row += nwarps) {
-    for (int h0 = 0; h0 < H; h0 += HPP) {
-      const int h = h0 + hq;
-      const bool act = h < H;
-      const long long off = (long long)row * HI + (act ? h : 0) * DH + sub * 8;
-      const uint4 a4 = *reinterpret_cast<const uint4*>(dog + off), b4 = *reinterpret_cast<const uint4*>(og + off);
-      const float sg = (act && gates) ? 1.f / (1.f + __expf(-gates[(long long)row * H + h])) : 1.f;
-      const uint32_t aw[4] = {a4.x, a4.y, a4.z, a4.w}, bw[4] = {b4.x, b4.y, b4.z, b4.w};
-      uint32_t ow[4];
-      float s = 0.f;
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 a = unpack2_bf16(aw[e]), b = unpack2_bf16(bw[e]);
-        s += a.x * b.x + a.y * b.y;
-        ow[e] = pack2_bf16(a.x * sg, a.y * sg);
-      }
-#pragma unroll
-      for (int o = 1; o < LPH; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      if (act) {
-        *reinterpret_cast<uint4*>(dop + off) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-        if (sub == 0) { dsum[(long long)h * M + row] = s; if (dsum_rowmajor) dsum_rowmajor[(long long)row * H + h] = s; }
-        if (dq_zero) {
-          *reinterpret_cast<float4*>(dq_zero + off) = make_float4(0.f, 0.f, 0.f, 0.f);
-          *reinterpret_cast<float4*>(dq_zero + off + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-    }
-  }
-}
+// ================================================================================================ backward, head dim 128
+// Same tile tables, span mask, soft-cap and gate as attn_bwd_k.
 
 // main pass: one CTA per (64-key tile, head), 8 warps.  At DH = 128 a warp cannot hold both the dK and the dV accumulators of its 16 keys
 // (2 x 64 fp32 per thread) next to the score fragments without spilling, so the two accumulators go to two warps: the warps of key group
@@ -835,6 +667,18 @@ int num_sms();
 using namespace tfx;
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 
+// tfx_attn_bwd_prep / tfx_attn_bwd_prep_d128; `name` is the entry point's name for error messages
+template <int DH>
+static int attn_bwd_prep(const char* name, const void* do_gated, const void* o_gated, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero,
+                         int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  long long blocks = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
+  long long cap = (long long)num_sms() * 8;
+  attn_bwd_prep_k<DH><<<(int)(blocks < cap ? blocks : cap), ROW_THREADS, 0, ST(stream)>>>((const __nv_bfloat16*)do_gated, (const __nv_bfloat16*)o_gated, gates,
+                                                                                         (__nv_bfloat16*)do_pre, dsum_hm, dsum_mh, dq_zero, M, H);
+  return check_launch(name);
+}
+
 extern "C" {
 
 int tfx_attn_fwd(const void* q, const void* k, const void* v, long long ld_q, long long ld_k, long long ld_v, const float* gates, int H,
@@ -842,18 +686,14 @@ int tfx_attn_fwd(const void* q, const void* k, const void* v, long long ld_q, lo
                  void* o, long long ld_o, float* lse, int M, float scale, float softcap, const float* skip_if_fast, void* stream) {
   if (n_tiles <= 0) return 0;
   TFX_REQUIRE(softcap > 0.f, "attn_fwd: softcap must be > 0 (got %f)", softcap);
-  attn_fwd_k<<<dim3(n_tiles, H), ATT_THREADS, 0, ST(stream)>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, ld_q, ld_k, ld_v, gates, H, kv_limit,
-                                                               tile_q0, tile_qend, tile_kv0, tile_kvend, (__nv_bfloat16*)o, ld_o, lse, M, scale, softcap, skip_if_fast);
+  attn_fwd_k<64><<<dim3(n_tiles, H), ATT_THREADS, 0, ST(stream)>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, ld_q, ld_k,
+                                                                                 ld_v, gates, H, kv_limit, tile_q0, tile_qend, tile_kv0, tile_kvend, (__nv_bfloat16*)o,
+                                                                                 ld_o, lse, M, scale, softcap, skip_if_fast);
   return check_launch("attn_fwd");
 }
 
 int tfx_attn_bwd_prep(const void* do_gated, const void* o_gated, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  long long blocks = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  long long cap = (long long)num_sms() * 8;
-  attn_bwd_prep_k<<<(int)(blocks < cap ? blocks : cap), ROW_THREADS, 0, ST(stream)>>>((const __nv_bfloat16*)do_gated, (const __nv_bfloat16*)o_gated, gates, (__nv_bfloat16*)do_pre,
-                                                                                   dsum_hm, dsum_mh, dq_zero, M, H);
-  return check_launch("attn_bwd_prep");
+  return attn_bwd_prep<64>("attn_bwd_prep", do_gated, o_gated, gates, do_pre, dsum_hm, dsum_mh, dq_zero, M, H, stream);
 }
 
 int tfx_attn_bwd(const void* q, const void* k, const void* v, const void* do_pre, long long ld_q, long long ld_k, long long ld_v, long long ld_do,
@@ -879,22 +719,17 @@ int tfx_attn_fwd_d128(const void* q, const void* k, const void* v, long long ld_
   TFX_REQUIRE(ld_q % 8 == 0 && ld_k % 8 == 0 && ld_v % 8 == 0 && ld_o % 2 == 0, "attn_fwd_d128: row pitches must keep 16-byte rows aligned");
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(attn_fwd_dh_k<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_FWD_SMEM_D128) != cudaSuccess) { set_error("attn_fwd_d128: cannot raise dynamic smem"); return -2; }
+    if (cudaFuncSetAttribute(attn_fwd_k<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, att_fwd_smem(128)) != cudaSuccess) { set_error("attn_fwd_d128: cannot raise dynamic smem"); return -2; }
     attr_set = true;
   }
-  attn_fwd_dh_k<128><<<dim3(n_tiles, H), ATT_THREADS, ATT_FWD_SMEM_D128, ST(stream)>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, ld_q, ld_k, ld_v,
+  attn_fwd_k<128><<<dim3(n_tiles, H), ATT_THREADS, att_fwd_smem(128), ST(stream)>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, ld_q, ld_k, ld_v,
                                                                                  gates, H, kv_limit, tile_q0, tile_qend, tile_kv0, tile_kvend, (__nv_bfloat16*)o, ld_o, lse, M,
-                                                                                 scale, softcap);
+                                                                                 scale, softcap, nullptr);
   return check_launch("attn_fwd_d128");
 }
 
 int tfx_attn_bwd_prep_d128(const void* do_gated, const void* o_gated, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  long long blocks = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  long long cap = (long long)num_sms() * 8;
-  attn_bwd_prep_dh_k<128><<<(int)(blocks < cap ? blocks : cap), ROW_THREADS, 0, ST(stream)>>>((const __nv_bfloat16*)do_gated, (const __nv_bfloat16*)o_gated, gates,
-                                                                                          (__nv_bfloat16*)do_pre, dsum_hm, dsum_mh, dq_zero, M, H);
-  return check_launch("attn_bwd_prep_d128");
+  return attn_bwd_prep<128>("attn_bwd_prep_d128", do_gated, o_gated, gates, do_pre, dsum_hm, dsum_mh, dq_zero, M, H, stream);
 }
 
 int tfx_attn_bwd_d128(const void* q, const void* k, const void* v, const void* do_pre, long long ld_q, long long ld_k, long long ld_v, long long ld_do,

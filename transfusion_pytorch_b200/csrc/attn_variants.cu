@@ -1,5 +1,6 @@
 // Optional attention variants of the reference's Attention.forward (transfusion.py:918-1039) as HBM-bound row kernels around the fused
-// attention kernels (one warp per token; 8 lanes share a head with 16-byte bf16 accesses, 4 heads per pass - the layout of attn_bwd_prep):
+// attention kernels (one warp per token; DH / 8 lanes share a head with 16-byte bf16 accesses, 32 / (DH / 8) heads per pass - the layout of
+// attn_bwd_prep).  The per-head kernels are templates on the head dim DH, instantiated at 64 and 128:
 //
 //   LASER (T.py:981-983, 1021-1022; laser_softclamp_value = 15):   v' = exp(15 tanh(v / 15))  ->  attention  ->  out = log(out) [* sigmoid(gate)]
 //       the kv cache keeps the RAW value (T.py:976-977 stacks before the transform); the transformed copy is a second slab written in place;
@@ -20,11 +21,13 @@ __device__ __forceinline__ float tanh_acc_v(float x) {          // abs err ~1e-7
 }
 __device__ __forceinline__ float sigmoid_v(float x) { return 1.f / (1.f + __expf(-x)); }
 
-#define VAR_ROW_LOOP                                                                                   \
-  const int lane = threadIdx.x & 31, sub = lane & 7, hq = lane >> 3;                                   \
+// One warp per token; DH / 8 lanes share a head (a lane owns 8 consecutive dims: 16-byte bf16 accesses), 32 / (DH / 8) heads per pass.
+#define VAR_ROW_LOOP(DH)                                                                               \
+  constexpr int LPH = (DH) / 8, HPP = 32 / LPH;                                                        \
+  const int lane = threadIdx.x & 31, sub = lane % LPH, hq = (lane >> 3) / (LPH / 8);                  \
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5; \
   for (int row = warp0; row < M; row += nwarps)                                                        \
-    for (int h0 = 0; h0 < H; h0 += 4)
+    for (int h0 = 0; h0 < H; h0 += HPP)
 
 __device__ __forceinline__ void ld8(const __nv_bfloat16* p, float (&x)[8]) {
   const uint4 t = *reinterpret_cast<const uint4*>(p);
@@ -34,15 +37,24 @@ __device__ __forceinline__ void ld8(const __nv_bfloat16* p, float (&x)[8]) {
 __device__ __forceinline__ void st8(__nv_bfloat16* p, const float (&x)[8]) {
   *reinterpret_cast<uint4*>(p) = make_uint4(pack2_bf16(x[0], x[1]), pack2_bf16(x[2], x[3]), pack2_bf16(x[4], x[5]), pack2_bf16(x[6], x[7]));
 }
-__device__ __forceinline__ float sum8lanes(float s) {
-  s += __shfl_xor_sync(0xffffffffu, s, 1); s += __shfl_xor_sync(0xffffffffu, s, 2); s += __shfl_xor_sync(0xffffffffu, s, 4);
+// sum over the LPH lanes of a head.  The same butterfly at both widths, spelled per width: each spelling keeps the generated code its width was
+// measured with (the loop form reschedules the 64-wide kernels, the unrolled form the 128-wide ones).
+template <int LPH>
+__device__ __forceinline__ float sum_head_lanes(float s) {
+  if constexpr (LPH == 8) {
+    s += __shfl_xor_sync(0xffffffffu, s, 1); s += __shfl_xor_sync(0xffffffffu, s, 2); s += __shfl_xor_sync(0xffffffffu, s, 4);
+  } else {
+#pragma unroll
+    for (int o = 1; o < LPH; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  }
   return s;
 }
 
+// laser_v_fwd / laser_v_bwd are elementwise and serve any head dim (a 128-wide head is two 64-wide ones).
 // v' = exp(c tanh(v / c)); rows (optional): cache row of token `row` (source and destination are then cache slabs)
 __global__ void __launch_bounds__(ROW_THREADS) laser_v_fwd_k(const __nv_bfloat16* __restrict__ v, long long ld_v, const int* __restrict__ rows, __nv_bfloat16* __restrict__ vl,
                                                             long long ld_vl, int M, int H, float c) {
-  VAR_ROW_LOOP {
+  VAR_ROW_LOOP(64) {
     const int h = h0 + hq;
     if (h >= H) continue;
     const long long r = rows ? rows[row] : row;
@@ -54,57 +66,9 @@ __global__ void __launch_bounds__(ROW_THREADS) laser_v_fwd_k(const __nv_bfloat16
   }
 }
 
-// att = log(o) * sigmoid(gate)
-__global__ void __launch_bounds__(ROW_THREADS) laser_out_fwd_k(const __nv_bfloat16* __restrict__ o, const float* __restrict__ gates, __nv_bfloat16* __restrict__ att, int M, int H) {
-  const long long HI = (long long)H * 64;
-  VAR_ROW_LOOP {
-    const int h = h0 + hq;
-    if (h >= H) continue;
-    const long long off = row * HI + h * 64 + sub * 8;
-    const float sg = gates ? sigmoid_v(gates[(long long)row * H + h]) : 1.f;
-    float x[8];
-    ld8(o + off, x);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) x[e] = __logf(fmaxf(x[e], 1e-30f)) * sg;
-    st8(att + off, x);
-  }
-}
-
-// backward of att = log(o) * sg:  dO = dAtt * sg / o ;  D[h][row] = sum_d dO * o = sum_d dAtt * sg ;  gate sums[row][h] = sum_d dAtt * att  (d gate_pre = (1 - sg) * that)
-__global__ void __launch_bounds__(ROW_THREADS) laser_bwd_prep_k(const __nv_bfloat16* __restrict__ datt, const __nv_bfloat16* __restrict__ o, const float* __restrict__ gates,
-                                                               __nv_bfloat16* __restrict__ dop, float* __restrict__ dsum, float* __restrict__ dsum_rowmajor, float* __restrict__ dq_zero,
-                                                               int M, int H) {
-  const long long HI = (long long)H * 64;
-  VAR_ROW_LOOP {
-    const int h = h0 + hq;
-    const bool act = h < H;
-    const long long off = row * HI + (act ? h : 0) * 64 + sub * 8;
-    const float sg = (act && gates) ? sigmoid_v(gates[(long long)row * H + h]) : 1.f;
-    float a[8], b[8], w[8];
-    ld8(datt + off, a); ld8(o + off, b);
-    float s = 0.f, gsum = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const float oo = fmaxf(b[e], 1e-30f);
-      s += a[e] * sg;
-      gsum += a[e] * __logf(oo) * sg;
-      w[e] = a[e] * sg / oo;
-    }
-    s = sum8lanes(s); gsum = sum8lanes(gsum);
-    if (act) {
-      st8(dop + off, w);
-      if (sub == 0) { dsum[(long long)h * M + row] = s; if (dsum_rowmajor) dsum_rowmajor[(long long)row * H + h] = gsum; }
-      if (dq_zero) {
-        *reinterpret_cast<float4*>(dq_zero + off) = make_float4(0.f, 0.f, 0.f, 0.f);
-        *reinterpret_cast<float4*>(dq_zero + off + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    }
-  }
-}
-
 // dv = dv' * v' * (1 - tanh^2(v / c)), in place on dv'
 __global__ void __launch_bounds__(ROW_THREADS) laser_v_bwd_k(__nv_bfloat16* __restrict__ dv, long long ld_dv, const __nv_bfloat16* __restrict__ v, long long ld_v, int M, int H, float c) {
-  VAR_ROW_LOOP {
+  VAR_ROW_LOOP(64) {
     const int h = h0 + hq;
     if (h >= H) continue;
     float g[8], x[8];
@@ -116,75 +80,11 @@ __global__ void __launch_bounds__(ROW_THREADS) laser_v_bwd_k(__nv_bfloat16* __re
   }
 }
 
-// v = v * mix + v0 * (1 - mix), in place; rows (optional) = cache row of the token in both v and v0
-__global__ void __launch_bounds__(ROW_THREADS) vmix_fwd_k(__nv_bfloat16* __restrict__ v, long long ld_v, const int* __restrict__ rows, const __nv_bfloat16* __restrict__ v0, long long ld_v0,
-                                                         const float* __restrict__ mixpre, const float* __restrict__ bias, int M, int H) {
-  VAR_ROW_LOOP {
-    const int h = h0 + hq;
-    if (h >= H) continue;
-    const long long r = rows ? rows[row] : row;
-    const float mix = sigmoid_v(mixpre[(long long)row * H + h] + bias[h]);
-    float a[8], b[8];
-    ld8(v + r * ld_v + h * 64 + sub * 8, a); ld8(v0 + r * ld_v0 + h * 64 + sub * 8, b);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) a[e] = a[e] * mix + b[e] * (1.f - mix);
-    st8(v + r * ld_v + h * 64 + sub * 8, a);
-  }
-}
-
-// backward of the mix (dv holds d v_mixed on entry, d v_raw on exit):  dv_raw = dvm * mix ;  dv0 += dvm * (1 - mix) ;
-// d mix_pre = sum_d dvm (v_raw - v0) mix (1 - mix) = sum_d dvm (v_mixed - v0) (1 - mix)        [v_mixed - v0 = (v_raw - v0) mix]
-__global__ void __launch_bounds__(ROW_THREADS) vmix_bwd_k(__nv_bfloat16* __restrict__ dv, long long ld_dv, const __nv_bfloat16* __restrict__ vm, long long ld_v,
-                                                         const __nv_bfloat16* __restrict__ v0, long long ld_v0, const float* __restrict__ mixpre, const float* __restrict__ bias,
-                                                         float* __restrict__ dv0_acc, __nv_bfloat16* __restrict__ dmix, long long ld_dmix, int M, int H) {
-  const long long HI = (long long)H * 64;
-  VAR_ROW_LOOP {
-    const int h = h0 + hq;
-    const bool act = h < H;
-    const int hh = act ? h : 0;
-    const float mix = sigmoid_v(mixpre[(long long)row * H + hh] + bias[hh]);
-    float g[8], a[8], b[8];
-    ld8(dv + (long long)row * ld_dv + hh * 64 + sub * 8, g);
-    ld8(vm + (long long)row * ld_v + hh * 64 + sub * 8, a);
-    ld8(v0 + (long long)row * ld_v0 + hh * 64 + sub * 8, b);
-    float s = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) s += g[e] * (a[e] - b[e]);
-    s = sum8lanes(s) * (1.f - mix);
-    if (act) {
-      float* acc = dv0_acc + row * HI + h * 64 + sub * 8;
-      const float4 c0 = *reinterpret_cast<const float4*>(acc), c1 = *reinterpret_cast<const float4*>(acc + 4);
-      const float om = 1.f - mix;
-      *reinterpret_cast<float4*>(acc) = make_float4(c0.x + g[0] * om, c0.y + g[1] * om, c0.z + g[2] * om, c0.w + g[3] * om);
-      *reinterpret_cast<float4*>(acc + 4) = make_float4(c1.x + g[4] * om, c1.y + g[5] * om, c1.z + g[6] * om, c1.w + g[7] * om);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) g[e] *= mix;
-      st8(dv + (long long)row * ld_dv + h * 64 + sub * 8, g);
-      if (sub == 0) dmix[(long long)row * ld_dmix + h] = __float2bfloat16(s);
-    }
-  }
-}
-
-// ---- head dim 128 (templates instantiated at 128 only; the 64-wide kernels above keep their own code): DH / 8 lanes per head (16 at 128),
-// 32 / (DH / 8) heads per pass.  laser_v_fwd / laser_v_bwd are elementwise and serve any head dim (a 128-wide head is two 64-wide ones).
-#define VAR_ROW_LOOP_DH                                                                                \
-  constexpr int LPH = DH / 8, HPP = 32 / LPH;                                                          \
-  const int lane = threadIdx.x & 31, sub = lane % LPH, hq = lane / LPH;                                \
-  const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5; \
-  for (int row = warp0; row < M; row += nwarps)                                                        \
-    for (int h0 = 0; h0 < H; h0 += HPP)
-
-template <int LPH>
-__device__ __forceinline__ float sum_head_lanes(float s) {
-#pragma unroll
-  for (int o = 1; o < LPH; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  return s;
-}
-
+// att = log(o) * sigmoid(gate)
 template <int DH>
-__global__ void __launch_bounds__(ROW_THREADS) laser_out_fwd_dh_k(const __nv_bfloat16* __restrict__ o, const float* __restrict__ gates, __nv_bfloat16* __restrict__ att, int M, int H) {
+__global__ void __launch_bounds__(ROW_THREADS) laser_out_fwd_k(const __nv_bfloat16* __restrict__ o, const float* __restrict__ gates, __nv_bfloat16* __restrict__ att, int M, int H) {
   const long long HI = (long long)H * DH;
-  VAR_ROW_LOOP_DH {
+  VAR_ROW_LOOP(DH) {
     const int h = h0 + hq;
     if (h >= H) continue;
     const long long off = row * HI + h * DH + sub * 8;
@@ -197,12 +97,13 @@ __global__ void __launch_bounds__(ROW_THREADS) laser_out_fwd_dh_k(const __nv_bfl
   }
 }
 
+// backward of att = log(o) * sg:  dO = dAtt * sg / o ;  D[h][row] = sum_d dO * o = sum_d dAtt * sg ;  gate sums[row][h] = sum_d dAtt * att  (d gate_pre = (1 - sg) * that)
 template <int DH>
-__global__ void __launch_bounds__(ROW_THREADS) laser_bwd_prep_dh_k(const __nv_bfloat16* __restrict__ datt, const __nv_bfloat16* __restrict__ o, const float* __restrict__ gates,
-                                                                  __nv_bfloat16* __restrict__ dop, float* __restrict__ dsum, float* __restrict__ dsum_rowmajor,
-                                                                  float* __restrict__ dq_zero, int M, int H) {
+__global__ void __launch_bounds__(ROW_THREADS) laser_bwd_prep_k(const __nv_bfloat16* __restrict__ datt, const __nv_bfloat16* __restrict__ o, const float* __restrict__ gates,
+                                                               __nv_bfloat16* __restrict__ dop, float* __restrict__ dsum, float* __restrict__ dsum_rowmajor,
+                                                               float* __restrict__ dq_zero, int M, int H) {
   const long long HI = (long long)H * DH;
-  VAR_ROW_LOOP_DH {
+  VAR_ROW_LOOP(DH) {
     const int h = h0 + hq;
     const bool act = h < H;
     const long long off = row * HI + (act ? h : 0) * DH + sub * 8;
@@ -229,10 +130,11 @@ __global__ void __launch_bounds__(ROW_THREADS) laser_bwd_prep_dh_k(const __nv_bf
   }
 }
 
+// v = v * mix + v0 * (1 - mix), in place; rows (optional) = cache row of the token in both v and v0
 template <int DH>
-__global__ void __launch_bounds__(ROW_THREADS) vmix_fwd_dh_k(__nv_bfloat16* __restrict__ v, long long ld_v, const int* __restrict__ rows, const __nv_bfloat16* __restrict__ v0,
-                                                            long long ld_v0, const float* __restrict__ mixpre, const float* __restrict__ bias, int M, int H) {
-  VAR_ROW_LOOP_DH {
+__global__ void __launch_bounds__(ROW_THREADS) vmix_fwd_k(__nv_bfloat16* __restrict__ v, long long ld_v, const int* __restrict__ rows, const __nv_bfloat16* __restrict__ v0,
+                                                         long long ld_v0, const float* __restrict__ mixpre, const float* __restrict__ bias, int M, int H) {
+  VAR_ROW_LOOP(DH) {
     const int h = h0 + hq;
     if (h >= H) continue;
     const long long r = rows ? rows[row] : row;
@@ -245,12 +147,14 @@ __global__ void __launch_bounds__(ROW_THREADS) vmix_fwd_dh_k(__nv_bfloat16* __re
   }
 }
 
+// backward of the mix (dv holds d v_mixed on entry, d v_raw on exit):  dv_raw = dvm * mix ;  dv0 += dvm * (1 - mix) ;
+// d mix_pre = sum_d dvm (v_raw - v0) mix (1 - mix) = sum_d dvm (v_mixed - v0) (1 - mix)        [v_mixed - v0 = (v_raw - v0) mix]
 template <int DH>
-__global__ void __launch_bounds__(ROW_THREADS) vmix_bwd_dh_k(__nv_bfloat16* __restrict__ dv, long long ld_dv, const __nv_bfloat16* __restrict__ vm, long long ld_v,
-                                                            const __nv_bfloat16* __restrict__ v0, long long ld_v0, const float* __restrict__ mixpre, const float* __restrict__ bias,
-                                                            float* __restrict__ dv0_acc, __nv_bfloat16* __restrict__ dmix, long long ld_dmix, int M, int H) {
+__global__ void __launch_bounds__(ROW_THREADS) vmix_bwd_k(__nv_bfloat16* __restrict__ dv, long long ld_dv, const __nv_bfloat16* __restrict__ vm, long long ld_v,
+                                                         const __nv_bfloat16* __restrict__ v0, long long ld_v0, const float* __restrict__ mixpre, const float* __restrict__ bias,
+                                                         float* __restrict__ dv0_acc, __nv_bfloat16* __restrict__ dmix, long long ld_dmix, int M, int H) {
   const long long HI = (long long)H * DH;
-  VAR_ROW_LOOP_DH {
+  VAR_ROW_LOOP(DH) {
     const int h = h0 + hq;
     const bool act = h < H;
     const int hh = act ? h : 0;
@@ -315,13 +219,13 @@ int tfx_laser_v_fwd(const void* v, long long ld_v, const int* rows, void* v_lase
 
 int tfx_laser_out_fwd(const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
   if (M <= 0) return 0;
-  laser_out_fwd_k<<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
+  laser_out_fwd_k<64><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
   return check_launch("laser_out_fwd");
 }
 
 int tfx_laser_bwd_prep(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
   if (M <= 0) return 0;
-  laser_bwd_prep_k<<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
+  laser_bwd_prep_k<64><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
   return check_launch("laser_bwd_prep");
 }
 
@@ -335,7 +239,7 @@ int tfx_laser_v_bwd(void* dv_inout, long long ld_dv, const void* v, long long ld
 int tfx_vmix_fwd(void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias, int M, int H, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && mix_pre && mix_bias, "vmix_fwd: bad arguments");
-  vmix_fwd_k<<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
+  vmix_fwd_k<64><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
   return check_launch("vmix_fwd");
 }
 
@@ -343,26 +247,26 @@ int tfx_vmix_bwd(void* dv_inout, long long ld_dv, const void* v_mixed, long long
                  float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && ld_dv % 8 == 0, "vmix_bwd: row pitches must be multiples of 8 bf16");
-  vmix_bwd_k<<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc, BF(dmix_bf16), ld_dmix, M, H);
+  vmix_bwd_k<64><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc, BF(dmix_bf16), ld_dmix, M, H);
   return check_launch("vmix_bwd");
 }
 
 int tfx_laser_out_fwd_d128(const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
   if (M <= 0) return 0;
-  laser_out_fwd_dh_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
+  laser_out_fwd_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
   return check_launch("laser_out_fwd_d128");
 }
 
 int tfx_laser_bwd_prep_d128(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
   if (M <= 0) return 0;
-  laser_bwd_prep_dh_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
+  laser_bwd_prep_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
   return check_launch("laser_bwd_prep_d128");
 }
 
 int tfx_vmix_fwd_d128(void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias, int M, int H, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && mix_pre && mix_bias, "vmix_fwd_d128: bad arguments");
-  vmix_fwd_dh_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
+  vmix_fwd_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
   return check_launch("vmix_fwd_d128");
 }
 
@@ -370,7 +274,7 @@ int tfx_vmix_bwd_d128(void* dv_inout, long long ld_dv, const void* v_mixed, long
                       float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && ld_dv % 8 == 0, "vmix_bwd_d128: row pitches must be multiples of 8 bf16");
-  vmix_bwd_dh_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc,
+  vmix_bwd_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc,
                                                                  BF(dmix_bf16), ld_dmix, M, H);
   return check_launch("vmix_bwd_d128");
 }

@@ -106,7 +106,8 @@ __global__ void __launch_bounds__(128) attn_decode_k(const __nv_bfloat16* __rest
   }
 }
 
-// head dim 128 (template, instantiated at 128 only; the 64-wide kernel above keeps its own code): lane <-> DH / 32 output dims for P V
+// head dim 128: lane <-> DH / 32 output dims for P V.  Instantiated at 128 only: the 64-wide kernel above keeps its own code, because this
+// template at DH = 64 (a uint32_t pair per lane) schedules differently and measured 0.2 % slower (129.6 vs 129.4 us per call, H100 80GB HBM3, 700 W).
 template <int DH>
 __global__ void __launch_bounds__(128) attn_decode_dh_k(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k, const __nv_bfloat16* __restrict__ v,
                                                        long long ld_q, long long ld_k, long long ld_v, const float* __restrict__ gates, int H, const int* __restrict__ kv_limit,

@@ -726,153 +726,19 @@ __global__ void __launch_bounds__(ROW_THREADS) clean_flow_bwd_k(float* __restric
 }
 
 // ------------------------------------------------------------------------------------ qk RMSNorm + RoPE backward, packs d[q|k|.|gates]
-// forward (GEMM epilogue): xhat = x*inv;  y = xhat*8*(gamma+1);  q = R(pos) y (interleaved pairs)   (T.py:950-965)
-// One warp per token; 8 lanes share a head (lane owns 8 consecutive dims = 4 rope pairs: 32 B fp32 / 16 B bf16 accesses),
-// so a warp covers 4 heads per pass and the per-head dot product is a 3-step shuffle.
-// xhat is rebuilt from the bf16 output as R^T q / (8 (gamma + 1)): where gamma_j = -1 the forward wrote y_j = 0 and xhat_j is lost, so
-// dx_j and dgamma_j come out 0 instead of -inv xhat_j (xhat . dxhat) and sum 8 dy_j xhat_j; near -1 the bf16 error of the rope partner is
-// amplified by |gamma_partner + 1| / |gamma_j + 1|.
+// forward (GEMM epilogue): xhat = x*inv;  y = xhat*sqrt(DH)*(gamma+1);  q = R(pos) y (interleaved pairs)   (T.py:950-965)
+// One warp per token; DH / 8 lanes share a head (8 at DH = 64, 16 at 128) and a lane owns 8 consecutive dims = 4 rope pairs (32 B fp32 /
+// 16 B bf16 accesses), so a warp covers 32 / (DH / 8) heads per pass and the per-head dot product is a log2(DH / 8)-step shuffle.
+// rope_cs is [pos][DH / 2] (cos, sin).
+// xhat is rebuilt from the bf16 output as R^T q / (sqrt(DH) (gamma + 1)): where gamma_j = -1 the forward wrote y_j = 0 and xhat_j is lost, so
+// dx_j and dgamma_j come out 0 instead of -inv xhat_j (xhat . dxhat) and sum sqrt(DH) dy_j xhat_j; near -1 the bf16 error of the rope partner
+// is amplified by |gamma_partner + 1| / |gamma_j + 1|.
+template <int DH>
 __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_k(const float* __restrict__ dq, const float* __restrict__ dk, const __nv_bfloat16* __restrict__ q,
                                                             const __nv_bfloat16* __restrict__ k, const float* __restrict__ qk_inv, const float* __restrict__ gq,
                                                             const float* __restrict__ gk, const int* __restrict__ rope_pos, const float2* __restrict__ rope_cs,
                                                             const float* __restrict__ gates, const float* __restrict__ dsum, __nv_bfloat16* __restrict__ out,
                                                             long long out_ld, float* __restrict__ dgq, float* __restrict__ dgk, int M, int H, int tpw) {
-  __shared__ float red[WARPS_PER_BLOCK][128];
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int sub = lane & 7, hq = lane >> 3;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);
-  const int HI = H * 64;
-  float acc[2][8];
-  float g1[2][8], rg[2][8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    acc[0][j] = acc[1][j] = 0.f;
-    g1[0][j] = gq[sub * 8 + j] + 1.f; g1[1][j] = gk[sub * 8 + j] + 1.f;
-    rg[0][j] = fabsf(g1[0][j]) > 1e-12f ? 1.f / (8.f * g1[0][j]) : 0.f;
-    rg[1][j] = fabsf(g1[1][j]) > 1e-12f ? 1.f / (8.f * g1[1][j]) : 0.f;
-  }
-  for (int row = r0; row < r1; ++row) {
-    float cs[8];   // (cos, sin) of the lane's 4 rope pairs
-    {
-      const float4* cp = reinterpret_cast<const float4*>(rope_cs + (long long)rope_pos[row] * 32 + sub * 4);
-      const float4 c0 = cp[0], c1 = cp[1];
-      cs[0] = c0.x; cs[1] = c0.y; cs[2] = c0.z; cs[3] = c0.w; cs[4] = c1.x; cs[5] = c1.y; cs[6] = c1.z; cs[7] = c1.w;
-    }
-    for (int h0 = 0; h0 < H; h0 += 4) {
-      const int h = h0 + hq;
-      const bool act = h < H;
-      const long long off = (long long)row * HI + (act ? h : 0) * 64 + sub * 8;
-      // all loads of this head group (q and k, gradient and value) are issued before any arithmetic
-      const float4 da[2] = {*reinterpret_cast<const float4*>(dq + off), *reinterpret_cast<const float4*>(dk + off)};
-      const float4 db[2] = {*reinterpret_cast<const float4*>(dq + off + 4), *reinterpret_cast<const float4*>(dk + off + 4)};
-      const uint4 tv[2] = {*reinterpret_cast<const uint4*>(q + off), *reinterpret_cast<const uint4*>(k + off)};
-      const float invs[2] = {act ? qk_inv[(long long)row * 2 * H + h] : 0.f, act ? qk_inv[(long long)row * 2 * H + H + h] : 0.f};
-#pragma unroll
-      for (int which = 0; which < 2; ++which) {
-        const float dr[8] = {da[which].x, da[which].y, da[which].z, da[which].w, db[which].x, db[which].y, db[which].z, db[which].w};
-        const float2 p0 = unpack2_bf16(tv[which].x), p1 = unpack2_bf16(tv[which].y), p2 = unpack2_bf16(tv[which].z), p3 = unpack2_bf16(tv[which].w);
-        const float r[8] = {p0.x, p0.y, p1.x, p1.y, p2.x, p2.y, p3.x, p3.y};
-        const float inv = invs[which];
-        float xh[8], dxh[8], dot = 0.f;
-#pragma unroll
-        for (int pr = 0; pr < 4; ++pr) {
-          const float c = cs[2 * pr], sn = cs[2 * pr + 1];
-          // un-rotate (R^T)
-          const float y0 = r[2 * pr] * c + r[2 * pr + 1] * sn, y1 = r[2 * pr + 1] * c - r[2 * pr] * sn;
-          const float dy0 = dr[2 * pr] * c + dr[2 * pr + 1] * sn, dy1 = dr[2 * pr + 1] * c - dr[2 * pr] * sn;
-          xh[2 * pr] = y0 * rg[which][2 * pr]; xh[2 * pr + 1] = y1 * rg[which][2 * pr + 1];
-          dxh[2 * pr] = dy0 * 8.f * g1[which][2 * pr]; dxh[2 * pr + 1] = dy1 * 8.f * g1[which][2 * pr + 1];
-          if (act) { acc[which][2 * pr] += dy0 * xh[2 * pr] * 8.f; acc[which][2 * pr + 1] += dy1 * xh[2 * pr + 1] * 8.f; }
-          dot += xh[2 * pr] * dxh[2 * pr] + xh[2 * pr + 1] * dxh[2 * pr + 1];
-        }
-        dot += __shfl_xor_sync(0xffffffffu, dot, 1); dot += __shfl_xor_sync(0xffffffffu, dot, 2); dot += __shfl_xor_sync(0xffffffffu, dot, 4);
-        if (act) {
-          uint32_t w[4];
-#pragma unroll
-          for (int pr = 0; pr < 4; ++pr) w[pr] = pack2_bf16(inv * (dxh[2 * pr] - xh[2 * pr] * dot), inv * (dxh[2 * pr + 1] - xh[2 * pr + 1] * dot));
-          *reinterpret_cast<uint4*>(out + (long long)row * out_ld + which * HI + h * 64 + sub * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-    }
-    // gate logits: d g = (1 - sigmoid(g)) * sum_d dO_gated * O_gated
-    if (lane < H) {
-      const float gl = gates[(long long)row * H + lane];
-      const float sg = 1.f / (1.f + __expf(-gl));
-      out[(long long)row * out_ld + 3 * HI + lane] = __float2bfloat16((1.f - sg) * dsum[(long long)row * H + lane]);
-    }
-  }
-  // gamma gradients: reduce the 4 head-groups of the warp, then the 8 warps of the block, then one atomic per column per block
-#pragma unroll
-  for (int which = 0; which < 2; ++which)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float v = acc[which][j];
-      v += __shfl_xor_sync(0xffffffffu, v, 8); v += __shfl_xor_sync(0xffffffffu, v, 16);
-      if (hq == 0) red[wib][which * 64 + sub * 8 + j] = v;
-    }
-  __syncthreads();
-  if (threadIdx.x < 128) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < WARPS_PER_BLOCK; ++w) t += red[w][threadIdx.x];
-    atomicAdd((threadIdx.x < 64 ? dgq : dgk) + (threadIdx.x & 63), t);
-  }
-}
-
-// ------------------------------------------------------------------------------------ RoPE backward (qk_rmsnorm = False), packs d[q|k|.|gates]
-// forward (GEMM epilogue EPI_QKVG_ROPE): q = R(pos) x.  d x = R(pos)^T d q per interleaved pair; no saved values are needed.  Same lane
-// layout as qk_bwd_pack_k: 8 lanes per head, a lane owns 8 consecutive dims (4 rope pairs), 4 heads per pass.
-__global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_rope_k(const float* __restrict__ dq, const float* __restrict__ dk, const int* __restrict__ rope_pos,
-                                                                 const float2* __restrict__ rope_cs, const float* __restrict__ gates, const float* __restrict__ dsum,
-                                                                 __nv_bfloat16* __restrict__ out, long long out_ld, int M, int H, int tpw) {
-  const int lane = threadIdx.x & 31;
-  const int sub = lane & 7, hq = lane >> 3;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);
-  const int HI = H * 64;
-  for (int row = r0; row < r1; ++row) {
-    float cs[8];   // (cos, sin) of the lane's 4 rope pairs
-    {
-      const float4* cp = reinterpret_cast<const float4*>(rope_cs + (long long)rope_pos[row] * 32 + sub * 4);
-      const float4 c0 = cp[0], c1 = cp[1];
-      cs[0] = c0.x; cs[1] = c0.y; cs[2] = c0.z; cs[3] = c0.w; cs[4] = c1.x; cs[5] = c1.y; cs[6] = c1.z; cs[7] = c1.w;
-    }
-    for (int h0 = 0; h0 < H; h0 += 4) {
-      const int h = h0 + hq;
-      if (h >= H) continue;
-      const long long off = (long long)row * HI + h * 64 + sub * 8;
-      const float4 da[2] = {*reinterpret_cast<const float4*>(dq + off), *reinterpret_cast<const float4*>(dk + off)};
-      const float4 db[2] = {*reinterpret_cast<const float4*>(dq + off + 4), *reinterpret_cast<const float4*>(dk + off + 4)};
-#pragma unroll
-      for (int which = 0; which < 2; ++which) {
-        const float dr[8] = {da[which].x, da[which].y, da[which].z, da[which].w, db[which].x, db[which].y, db[which].z, db[which].w};
-        uint32_t w[4];
-#pragma unroll
-        for (int pr = 0; pr < 4; ++pr) {
-          const float c = cs[2 * pr], sn = cs[2 * pr + 1];
-          w[pr] = pack2_bf16(dr[2 * pr] * c + dr[2 * pr + 1] * sn, dr[2 * pr + 1] * c - dr[2 * pr] * sn);     // un-rotate (R^T)
-        }
-        *reinterpret_cast<uint4*>(out + (long long)row * out_ld + which * HI + h * 64 + sub * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-      }
-    }
-    // gate logits: d g = (1 - sigmoid(g)) * sum_d dO_gated * O_gated  (as in qk_bwd_pack_k)
-    if (lane < H) {
-      const float gl = gates[(long long)row * H + lane];
-      const float sg = 1.f / (1.f + __expf(-gl));
-      out[(long long)row * out_ld + 3 * HI + lane] = __float2bfloat16((1.f - sg) * dsum[(long long)row * H + lane]);
-    }
-  }
-}
-
-// ---- head dim 128 (templates instantiated at 128 only; the 64-wide kernels above keep their own code): DH / 8 lanes per head (a lane still
-// owns 8 consecutive dims = 4 rope pairs), 32 / (DH / 8) heads per pass; the norm scale is sqrt(DH); rope_cs is [pos][DH / 2] (cos, sin)
-template <int DH>
-__global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_dh_k(const float* __restrict__ dq, const float* __restrict__ dk, const __nv_bfloat16* __restrict__ q,
-                                                               const __nv_bfloat16* __restrict__ k, const float* __restrict__ qk_inv, const float* __restrict__ gq,
-                                                               const float* __restrict__ gk, const int* __restrict__ rope_pos, const float2* __restrict__ rope_cs,
-                                                               const float* __restrict__ gates, const float* __restrict__ dsum, __nv_bfloat16* __restrict__ out,
-                                                               long long out_ld, float* __restrict__ dgq, float* __restrict__ dgk, int M, int H, int tpw) {
   constexpr int LPH = DH / 8, HPP = 32 / LPH;
   static_assert(2 * DH <= ROW_THREADS, "one thread per gamma column in the block reduction");
   const float RS = sqrtf((float)DH);
@@ -902,6 +768,7 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_dh_k(const float* __r
       const int h = h0 + hq;
       const bool act = h < H;
       const long long off = (long long)row * HI + (act ? h : 0) * DH + sub * 8;
+      // all loads of this head group (q and k, gradient and value) are issued before any arithmetic
       const float4 da[2] = {*reinterpret_cast<const float4*>(dq + off), *reinterpret_cast<const float4*>(dk + off)};
       const float4 db[2] = {*reinterpret_cast<const float4*>(dq + off + 4), *reinterpret_cast<const float4*>(dk + off + 4)};
       const uint4 tv[2] = {*reinterpret_cast<const uint4*>(q + off), *reinterpret_cast<const uint4*>(k + off)};
@@ -916,6 +783,7 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_dh_k(const float* __r
 #pragma unroll
         for (int pr = 0; pr < 4; ++pr) {
           const float c = cs[2 * pr], sn = cs[2 * pr + 1];
+          // un-rotate (R^T)
           const float y0 = r[2 * pr] * c + r[2 * pr + 1] * sn, y1 = r[2 * pr + 1] * c - r[2 * pr] * sn;
           const float dy0 = dr[2 * pr] * c + dr[2 * pr + 1] * sn, dy1 = dr[2 * pr + 1] * c - dr[2 * pr] * sn;
           xh[2 * pr] = y0 * rg[which][2 * pr]; xh[2 * pr + 1] = y1 * rg[which][2 * pr + 1];
@@ -933,6 +801,7 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_dh_k(const float* __r
         }
       }
     }
+    // gate logits: d g = (1 - sigmoid(g)) * sum_d dO_gated * O_gated
     if (lane < H) {
       const float gl = gates[(long long)row * H + lane];
       const float sg = 1.f / (1.f + __expf(-gl));
@@ -958,10 +827,13 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_dh_k(const float* __r
   }
 }
 
+// ------------------------------------------------------------------------------------ RoPE backward (qk_rmsnorm = False), packs d[q|k|.|gates]
+// forward (GEMM epilogue EPI_QKVG_ROPE): q = R(pos) x.  d x = R(pos)^T d q per interleaved pair; no saved values are needed.  Same lane
+// layout as qk_bwd_pack_k.
 template <int DH>
-__global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_rope_dh_k(const float* __restrict__ dq, const float* __restrict__ dk, const int* __restrict__ rope_pos,
-                                                                    const float2* __restrict__ rope_cs, const float* __restrict__ gates, const float* __restrict__ dsum,
-                                                                    __nv_bfloat16* __restrict__ out, long long out_ld, int M, int H, int tpw) {
+__global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_rope_k(const float* __restrict__ dq, const float* __restrict__ dk, const int* __restrict__ rope_pos,
+                                                                 const float2* __restrict__ rope_cs, const float* __restrict__ gates, const float* __restrict__ dsum,
+                                                                 __nv_bfloat16* __restrict__ out, long long out_ld, int M, int H, int tpw) {
   constexpr int LPH = DH / 8, HPP = 32 / LPH;
   const int lane = threadIdx.x & 31;
   const int sub = lane % LPH, hq = lane / LPH;
@@ -969,7 +841,7 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_rope_dh_k(const float
   const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);
   const int HI = H * DH;
   for (int row = r0; row < r1; ++row) {
-    float cs[8];
+    float cs[8];   // (cos, sin) of the lane's 4 rope pairs
     {
       const float4* cp = reinterpret_cast<const float4*>(rope_cs + (long long)rope_pos[row] * (DH / 2) + sub * 4);
       const float4 c0 = cp[0], c1 = cp[1];
@@ -993,6 +865,7 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_rope_dh_k(const float
         *reinterpret_cast<uint4*>(out + (long long)row * out_ld + which * HI + h * DH + sub * 8) = make_uint4(w[0], w[1], w[2], w[3]);
       }
     }
+    // gate logits: d g = (1 - sigmoid(g)) * sum_d dO_gated * O_gated  (as in qk_bwd_pack_k)
     if (lane < H) {
       const float gl = gates[(long long)row * H + lane];
       const float sg = 1.f / (1.f + __expf(-gl));
@@ -1191,7 +1064,7 @@ int tfx_qk_bwd_pack(const float* dq, const float* dk, const void* q_bf16, const 
   if (M <= 0) return 0;
   TFX_REQUIRE(H >= 1 && H <= 32, "qk_bwd_pack: heads %d out of range", H);
   const int tpw = 8;
-  qk_bwd_pack_k<<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, (const __nv_bfloat16*)q_bf16, (const __nv_bfloat16*)k_bf16, qk_inv, q_gamma, k_gamma, rope_pos,
+  qk_bwd_pack_k<64><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, (const __nv_bfloat16*)q_bf16, (const __nv_bfloat16*)k_bf16, qk_inv, q_gamma, k_gamma, rope_pos,
                                                                      (const float2*)rope_cs, gates, dsum, (__nv_bfloat16*)dqkvg_bf16, out_ld, dq_gamma, dk_gamma, M, H, tpw);
   return check_launch("qk_bwd_pack");
 }
@@ -1201,7 +1074,7 @@ int tfx_qk_bwd_pack_rope(const float* dq, const float* dk, const int* rope_pos, 
   if (M <= 0) return 0;
   TFX_REQUIRE(H >= 1 && H <= 32, "qk_bwd_pack_rope: heads %d out of range", H);
   const int tpw = 8;
-  qk_bwd_pack_rope_k<<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, rope_pos, (const float2*)rope_cs, gates, dsum_mh, (__nv_bfloat16*)dqkvg_bf16, out_ld, M, H, tpw);
+  qk_bwd_pack_rope_k<64><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, rope_pos, (const float2*)rope_cs, gates, dsum_mh, (__nv_bfloat16*)dqkvg_bf16, out_ld, M, H, tpw);
   return check_launch("qk_bwd_pack_rope");
 }
 
@@ -1211,7 +1084,7 @@ int tfx_qk_bwd_pack_d128(const float* dq, const float* dk, const void* q_bf16, c
   if (M <= 0) return 0;
   TFX_REQUIRE(H >= 1 && H <= 16, "qk_bwd_pack_d128: heads %d out of range [1, 16]", H);
   const int tpw = 8;
-  qk_bwd_pack_dh_k<128><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, (const __nv_bfloat16*)q_bf16, (const __nv_bfloat16*)k_bf16, qk_inv, q_gamma, k_gamma,
+  qk_bwd_pack_k<128><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, (const __nv_bfloat16*)q_bf16, (const __nv_bfloat16*)k_bf16, qk_inv, q_gamma, k_gamma,
                                                                            rope_pos, (const float2*)rope_cs, gates, dsum, (__nv_bfloat16*)dqkvg_bf16, out_ld, dq_gamma,
                                                                            dk_gamma, M, H, tpw);
   return check_launch("qk_bwd_pack_d128");
@@ -1222,7 +1095,7 @@ int tfx_qk_bwd_pack_rope_d128(const float* dq, const float* dk, const int* rope_
   if (M <= 0) return 0;
   TFX_REQUIRE(H >= 1 && H <= 16, "qk_bwd_pack_rope_d128: heads %d out of range [1, 16]", H);
   const int tpw = 8;
-  qk_bwd_pack_rope_dh_k<128><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, rope_pos, (const float2*)rope_cs, gates, dsum_mh, (__nv_bfloat16*)dqkvg_bf16,
+  qk_bwd_pack_rope_k<128><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, rope_pos, (const float2*)rope_cs, gates, dsum_mh, (__nv_bfloat16*)dqkvg_bf16,
                                                                                 out_ld, M, H, tpw);
   return check_launch("qk_bwd_pack_rope_d128");
 }
