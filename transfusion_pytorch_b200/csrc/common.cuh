@@ -83,7 +83,7 @@ __device__ __forceinline__ void cp_async_4(uint32_t dst, const void* src) { asm 
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 
-// dispatch on model dim D = 128 * NCH: 128, 256, 384, 512, 768 or 1024 (transfusion.py MODEL_DIMS lists the same widths)
+// dispatch on model dim D = 128 * NCH: 128, 256, 384, 512, 768, 1024, 1536 or 2048 (transfusion.py MODEL_DIMS lists the same widths)
 #define TFX_DISPATCH_NCH(D, ...)                                                       \
   do {                                                                                 \
     switch ((D) / 128) {                                                               \
@@ -93,7 +93,9 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
       case 4: { constexpr int NCH = 4; __VA_ARGS__; } break;                           \
       case 6: { constexpr int NCH = 6; __VA_ARGS__; } break;                           \
       case 8: { constexpr int NCH = 8; __VA_ARGS__; } break;                           \
-      default: tfx::set_error("unsupported model dim %d (need 128, 256, 384, 512, 768 or 1024)", (int)(D)); return -1; \
+      case 12: { constexpr int NCH = 12; __VA_ARGS__; } break;                         \
+      case 16: { constexpr int NCH = 16; __VA_ARGS__; } break;                         \
+      default: tfx::set_error("unsupported model dim %d (need 128, 256, 384, 512, 768, 1024, 1536 or 2048)", (int)(D)); return -1; \
     }                                                                                  \
   } while (0)
 

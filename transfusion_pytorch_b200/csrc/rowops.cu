@@ -13,19 +13,29 @@ namespace tfx {
 constexpr int MAX_HIDDENS = TFX_MAX_DEPTH + 1;    // x0 and every layer output: 65 pointers, 520 B of kernel parameters
 struct HiddenList { const __nv_bfloat16* p[MAX_HIDDENS]; };
 
+// Wide rows (D = 1536, 2048: NCH 12, 16).  The lane layout stays the same, but a whole row per lane (48 / 64 floats per array) no longer fits
+// in registers next to the other rows a kernel holds.  The kernels that would spill take such rows in groups of WIDE_GROUP chunks
+// (512 columns, 16 floats per lane) instead: a row reduction is one pass over the groups, and the apply pass reads each group again - from
+// the row's cp.async ring slot where the kernel has one, else from global memory, where the row was just read and is still cached.
+// Per-column accumulators that outlive a row live in per-warp shared-memory rows; a lane only touches its own columns there, so no barrier
+// is needed.  Every kernel with NCH <= 8 keeps its register-row form.
+constexpr int WIDE_GROUP = 4;
+
 // ------------------------------------------------------------------------------------ adaLN forward
 // u = isM ? LN(x)*(gamma_c+1)+beta_c : LN(x)*(g+1)      (T.py:747-755; text-only 677-679)
 // The fp32 token rows stream through a per-warp ring of shared-memory slots filled by lane-private cp.async pieces (ADALN_FWD_RING - 1 rows per
 // warp in flight, no registers spent) - with one row per warp in flight the loads are latency-bound.
 // The FiLM rows (L2-resident, address depends on the token's condition row) are plain loads; the condition row is fetched one row ahead.
-constexpr int ADALN_FWD_RING = 4;
+// Wide rows (NCH > 8, see WIDE_GROUP) are not copied to registers: the mean, variance and apply passes each read the row's ring slot in
+// 512-column groups, and the slot is refilled after the apply pass.  Three 8 KB slots per warp keep the ring within 227 KB at D = 2048.
+template <int NCH> constexpr int ADALN_FWD_RING = NCH > 8 ? 3 : 4;
 template <int NCH>
 __global__ void __launch_bounds__(ROW_THREADS) adaln_fwd_k(const float* __restrict__ x, const int* __restrict__ cond_row,
                                                           const float* __restrict__ film, long long film_ld,
                                                           const float* __restrict__ g, __nv_bfloat16* __restrict__ u,
                                                           float* __restrict__ stats, int M) {
   constexpr int D = NCH * 128;
-  constexpr int RING = ADALN_FWD_RING;
+  constexpr int RING = ADALN_FWD_RING<NCH>;
   const int lane = threadIdx.x & 31;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   extern __shared__ __align__(16) float adaln_ring[];
@@ -45,6 +55,52 @@ __global__ void __launch_bounds__(ROW_THREADS) adaln_fwd_k(const float* __restri
 #pragma unroll
   for (int i = 0; i < RING; ++i) issue();
   int cons_slot = 0;
+  if constexpr (NCH > 8) {
+    constexpr int W = WIDE_GROUP;
+    int cr_next = (cond_row && warp0 < M) ? cond_row[warp0] : -1;
+    for (int row = warp0; row < M; row += nwarps) {
+      const int cr = cr_next;
+      cr_next = (cond_row && row + nwarps < M) ? cond_row[row + nwarps] : -1;
+      cp_async_wait<RING - 1>();
+      const float* xs = ring + cons_slot * D;
+      float v[W * 4], s = 0.f, q = 0.f;
+#pragma unroll 1
+      for (int c0 = 0; c0 < NCH; c0 += W) {
+        load_row_f32<W>(xs + c0 * 128, lane, v);
+#pragma unroll
+        for (int i = 0; i < W * 4; ++i) s += v[i];
+      }
+      const float mean = warp_sum(s) * (1.f / D);
+#pragma unroll 1
+      for (int c0 = 0; c0 < NCH; c0 += W) {
+        load_row_f32<W>(xs + c0 * 128, lane, v);
+#pragma unroll
+        for (int i = 0; i < W * 4; ++i) { v[i] -= mean; q += v[i] * v[i]; }
+      }
+      const float rstd = rsqrtf(warp_sum(q) * (1.f / D) + 1e-5f);
+#pragma unroll 1
+      for (int c0 = 0; c0 < NCH; c0 += W) {
+        float sc[W * 4], bt[W * 4];
+        load_row_f32<W>(xs + c0 * 128, lane, v);
+        if (cr >= 0) {
+          load_row_f32<W>(film + cr * film_ld + c0 * 128, lane, sc);
+          load_row_f32<W>(film + cr * film_ld + D + c0 * 128, lane, bt);
+#pragma unroll
+          for (int i = 0; i < W * 4; ++i) v[i] = (v[i] - mean) * rstd * (sc[i] + 1.f) + bt[i];
+        } else {
+          load_row_f32<W>(g + c0 * 128, lane, sc);
+#pragma unroll
+          for (int i = 0; i < W * 4; ++i) v[i] = (v[i] - mean) * rstd * (sc[i] + 1.f);
+        }
+        store_row_bf16<W>(u + (long long)row * D + c0 * 128, lane, v);
+      }
+      cons_slot = cons_slot + 1 == RING ? 0 : cons_slot + 1;
+      issue();
+      if (lane == 0) { stats[2 * row] = mean; stats[2 * row + 1] = rstd; }
+    }
+    cp_async_wait<0>();
+    return;
+  }
   float gv[NCH * 4];
   load_row_f32<NCH>(g, lane, gv);
   int cr_next = (cond_row && warp0 < M) ? cond_row[warp0] : -1;
@@ -95,6 +151,93 @@ __global__ void __launch_bounds__(ROW_THREADS, 2) adaln_bwd_k(const float* __res
   const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);      // (no early return: block-wide barrier below)
   // text rows all update the same [D] vector: per-warp smem rows + one block-level reduction instead of one global atomic per warp
   // (thousands of same-address atomics serialise in the L2 atomic units).  Condition rows are shared by only a few warps: direct red.
+  if constexpr (NCH > 8) {
+    // wide: one pass for m1, m2 and a second that reads du / x / the scale again and applies; the per-warp accumulators are shared-memory
+    // rows [d(gamma_c) | d(beta_c) of the current condition row | d(g) of the text rows], 3 x D floats per warp (dynamic, 192 KB at 2048)
+    constexpr int W = WIDE_GROUP;
+    extern __shared__ __align__(16) float adaln_bwd_acc[];
+    float* accA = adaln_bwd_acc + (threadIdx.x >> 5) * 3 * D;
+    float* accB = accA + D;
+    float* my_g = accB + D;
+    float z[W * 4];
+#pragma unroll
+    for (int i = 0; i < W * 4; ++i) z[i] = 0.f;
+#pragma unroll 1
+    for (int c0 = 0; c0 < NCH; c0 += W) store_row_f32<W>(my_g + c0 * 128, lane, z);
+    int cur = -1;
+    for (int row = r0; row < r1; ++row) {
+      const int cr = cond_row ? cond_row[row] : -1;
+      if (cr != cur) {
+#pragma unroll 1
+        for (int c0 = 0; c0 < NCH; c0 += W) {
+          float a[W * 4];
+          if (cur >= 0) {
+            load_row_f32<W>(accA + c0 * 128, lane, a); red_row_f32<W>(dfilm + cur * dfilm_ld + c0 * 128, lane, a);
+            load_row_f32<W>(accB + c0 * 128, lane, a); red_row_f32<W>(dfilm + cur * dfilm_ld + D + c0 * 128, lane, a);
+          }
+          store_row_f32<W>(accA + c0 * 128, lane, z); store_row_f32<W>(accB + c0 * 128, lane, z);
+        }
+        cur = cr;
+      }
+      const float mean = stats[2 * row], rstd = stats[2 * row + 1];
+      const float* scale = cr >= 0 ? film + cr * film_ld : g;
+      const float* dur = du + (long long)row * D;
+      const float* xr = x + (long long)row * D;
+      float m1 = 0.f, m2 = 0.f;
+#pragma unroll 1
+      for (int c0 = 0; c0 < NCH; c0 += W) {
+        float d[W * 4], xh[W * 4], sc[W * 4];
+        load_row_f32<W>(dur + c0 * 128, lane, d);
+        load_row_f32<W>(xr + c0 * 128, lane, xh);
+        load_row_f32<W>(scale + c0 * 128, lane, sc);
+#pragma unroll
+        for (int i = 0; i < W * 4; ++i) {
+          xh[i] = (xh[i] - mean) * rstd;
+          d[i] *= sc[i] + 1.f;
+          m1 += d[i]; m2 += d[i] * xh[i];
+        }
+      }
+      m1 = warp_sum(m1) * (1.f / D); m2 = warp_sum(m2) * (1.f / D);
+      float* acc = cr >= 0 ? accA : my_g;
+#pragma unroll 1
+      for (int c0 = 0; c0 < NCH; c0 += W) {
+        float d[W * 4], xh[W * 4], sc[W * 4], a[W * 4];
+        load_row_f32<W>(dur + c0 * 128, lane, d);
+        load_row_f32<W>(xr + c0 * 128, lane, xh);
+        load_row_f32<W>(scale + c0 * 128, lane, sc);
+        load_row_f32<W>(acc + c0 * 128, lane, a);
+#pragma unroll
+        for (int i = 0; i < W * 4; ++i) { xh[i] = (xh[i] - mean) * rstd; a[i] += d[i] * xh[i]; }
+        store_row_f32<W>(acc + c0 * 128, lane, a);
+        if (cr >= 0) {
+          load_row_f32<W>(accB + c0 * 128, lane, a);
+#pragma unroll
+          for (int i = 0; i < W * 4; ++i) a[i] += d[i];
+          store_row_f32<W>(accB + c0 * 128, lane, a);
+        }
+        load_row_f32<W>(dx + (long long)row * D + c0 * 128, lane, a);
+#pragma unroll
+        for (int i = 0; i < W * 4; ++i) a[i] += rstd * (d[i] * (sc[i] + 1.f) - m1 - xh[i] * m2);
+        store_row_f32<W>(dx + (long long)row * D + c0 * 128, lane, a);
+      }
+    }
+    if (cur >= 0) {
+#pragma unroll 1
+      for (int c0 = 0; c0 < NCH; c0 += W) {
+        float a[W * 4];
+        load_row_f32<W>(accA + c0 * 128, lane, a); red_row_f32<W>(dfilm + cur * dfilm_ld + c0 * 128, lane, a);
+        load_row_f32<W>(accB + c0 * 128, lane, a); red_row_f32<W>(dfilm + cur * dfilm_ld + D + c0 * 128, lane, a);
+      }
+    }
+    __syncthreads();
+    for (int c = threadIdx.x; c < D; c += ROW_THREADS) {
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < WARPS_PER_BLOCK; ++w) t += adaln_bwd_acc[w * 3 * D + 2 * D + c];
+      if (t != 0.f) atomicAdd(dg + c, t);
+    }
+    return;
+  }
   __shared__ __align__(16) float red_g[WARPS_PER_BLOCK][D];
   float* my_g = red_g[threadIdx.x >> 5];
   {
@@ -188,52 +331,59 @@ __global__ void __launch_bounds__(ROW_THREADS) resid_bwd_k(const float* __restri
                                                           float* __restrict__ dzgate, long long dzgate_ld, float* __restrict__ dls,
                                                           float* __restrict__ dbias, int M, int tpw) {
   constexpr int D = NCH * 128;
+  // every column is independent here, so a wide row is taken one 512-column group at a time, each group over all of the warp's rows
+  // (one group of NCH chunks up to NCH = 8)
+  constexpr int W = NCH > 8 ? WIDE_GROUP : NCH;
   extern __shared__ float red_smem[];
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);
   const bool has_scale = ls != nullptr;
-  float lsv[NCH * 4];
-  if (has_scale) load_row_f32<NCH>(ls, lane, lsv);
-  float acc[NCH * 4], accb[NCH * 4], accl[NCH * 4];      // per cond row / bias / layerscale (text rows) accumulators
+#pragma unroll 1
+  for (int c0 = 0; c0 < NCH; c0 += W) {
+    float lsv[W * 4];
+    if (has_scale) load_row_f32<W>(ls + c0 * 128, lane, lsv);
+    float acc[W * 4], accb[W * 4], accl[W * 4];      // per cond row / bias / layerscale (text rows) accumulators
 #pragma unroll
-  for (int i = 0; i < NCH * 4; ++i) { accb[i] = 0.f; accl[i] = 0.f; }
-  int cur = -2;
-  auto flush = [&]() {
-    if (cur == -2 || !has_scale) return;
-    if (cur >= 0) red_row_f32<NCH>(dzgate + cur * dzgate_ld, lane, acc);
-    else {
+    for (int i = 0; i < W * 4; ++i) { accb[i] = 0.f; accl[i] = 0.f; }
+    int cur = -2;
+    auto flush = [&]() {
+      if (cur == -2 || !has_scale) return;
+      if (cur >= 0) red_row_f32<W>(dzgate + cur * dzgate_ld + c0 * 128, lane, acc);
+      else {
 #pragma unroll
-      for (int i = 0; i < NCH * 4; ++i) accl[i] += acc[i];
-    }
-  };
-  for (int row = r0; row < r1; ++row) {
-    const int cr = (cond_row && zgate) ? cond_row[row] : -1;
-    if (cr != cur) {
-      flush(); cur = cr;
-#pragma unroll
-      for (int i = 0; i < NCH * 4; ++i) acc[i] = 0.f;
-    }
-    float d[NCH * 4];
-    load_row_f32<NCH>(dx + (long long)row * D, lane, d);
-    if (has_scale) {
-      float yv[NCH * 4], sc[NCH * 4];
-      load_row_bf16<NCH>(y + (long long)row * D, lane, yv);
-      if (cr >= 0) load_row_f32<NCH>(zgate + cr * zgate_ld, lane, sc);
-#pragma unroll
-      for (int i = 0; i < NCH * 4; ++i) {
-        const float s = cr >= 0 ? sc[i] : lsv[i] + 1.f;
-        acc[i] += d[i] * yv[i];
-        d[i] *= s;
+        for (int i = 0; i < W * 4; ++i) accl[i] += acc[i];
       }
-    }
+    };
+    for (int row = r0; row < r1; ++row) {
+      const int cr = (cond_row && zgate) ? cond_row[row] : -1;
+      if (cr != cur) {
+        flush(); cur = cr;
 #pragma unroll
-    for (int i = 0; i < NCH * 4; ++i) accb[i] += d[i];
-    store_row_bf16<NCH>(dy + (long long)row * D, lane, d);
+        for (int i = 0; i < W * 4; ++i) acc[i] = 0.f;
+      }
+      float d[W * 4];
+      load_row_f32<W>(dx + (long long)row * D + c0 * 128, lane, d);
+      if (has_scale) {
+        float yv[W * 4], sc[W * 4];
+        load_row_bf16<W>(y + (long long)row * D + c0 * 128, lane, yv);
+        if (cr >= 0) load_row_f32<W>(zgate + cr * zgate_ld + c0 * 128, lane, sc);
+#pragma unroll
+        for (int i = 0; i < W * 4; ++i) {
+          const float s = cr >= 0 ? sc[i] : lsv[i] + 1.f;
+          acc[i] += d[i] * yv[i];
+          d[i] *= s;
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < W * 4; ++i) accb[i] += d[i];
+      store_row_bf16<W>(dy + (long long)row * D + c0 * 128, lane, d);
+    }
+    flush();
+    if (dbias) block_red_cols<W>(red_smem, accb, dbias + c0 * 128);     // uniform branch: every thread of the block reaches the barrier
+    if (has_scale) { __syncthreads(); block_red_cols<W>(red_smem, accl, dls + c0 * 128); }   // layerscale gradient: one atomic per column per block
+    if (NCH > W) __syncthreads();                     // the next group reuses red_smem
   }
-  flush();
-  if (dbias) block_red_cols<NCH>(red_smem, accb, dbias);     // uniform branch: every thread of the block reaches the barrier
-  if (has_scale) { __syncthreads(); block_red_cols<NCH>(red_smem, accl, dls); }   // layerscale gradient: one atomic per column per block
 }
 
 // ------------------------------------------------------------------------------------ AttentionResidual forward
@@ -335,10 +485,11 @@ struct ResBwd2Args {
 // pieces: a lane only ever reads back what it copied itself, so cp.async.wait_group is the only synchronisation).  The item order of a row is
 // fixed - [scalars of the later layers + lse] [dx_out] [x_out] [h_0 .. h_{L1-1}] [dx_later ..] - so RING - 1 row loads per warp are always in
 // flight (a register prefetch keeps only one).
-template <int NCH> struct ResBwd2Cfg { static constexpr int RING = NCH <= 4 ? 5 : 3; };
+// Wide rows (NCH > 8) take RING = 2: the shared memory at D = 2048 is 8 KB (w of the own layer) + 64 KB (accumulators, below) + 128 KB (rings).
+template <int NCH> struct ResBwd2Cfg { static constexpr int RING = NCH <= 4 ? 5 : (NCH <= 8 ? 3 : 2); };
 
 template <int NCH, bool ACC>
-__global__ void __launch_bounds__(ROW_THREADS, 2) attn_res_bwd2_k(ResBwd2Args A, const float* __restrict__ dxo, const float* __restrict__ xo, const float* __restrict__ lse,
+__global__ void __launch_bounds__(ROW_THREADS, NCH > 8 ? 1 : 2) attn_res_bwd2_k(ResBwd2Args A, const float* __restrict__ dxo, const float* __restrict__ xo, const float* __restrict__ lse,
                                                                  float* __restrict__ G, float* __restrict__ sc_out, int sc_stride, float* __restrict__ partials, int M, int tpw) {
   constexpr int D = NCH * 128;
   constexpr int RING = ResBwd2Cfg<NCH>::RING;
@@ -347,7 +498,8 @@ __global__ void __launch_bounds__(ROW_THREADS, 2) attn_res_bwd2_k(ResBwd2Args A,
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);    // (no early return: block-wide barriers below)
   extern __shared__ __align__(16) float w_s[];                  // [max(1 + n_later, warps)][D]: w = (gamma + 1) * pq of the own layer (slot 0) and of the later ones; then the rings
-  const int w_slots = (1 + A.n_later) > WARPS_PER_BLOCK ? (1 + A.n_later) : WARPS_PER_BLOCK;
+  // (wide rows: [w of the own layer][accw: warps][rings], see below)
+  const int w_slots = NCH > 8 ? 1 + WARPS_PER_BLOCK : ((1 + A.n_later) > WARPS_PER_BLOCK ? (1 + A.n_later) : WARPS_PER_BLOCK);
   const uint8_t* ring = reinterpret_cast<const uint8_t*>(w_s + w_slots * D) + (threadIdx.x >> 5) * (RING * SLOT);
   const uint32_t ring_u32 = (uint32_t)__cvta_generic_to_shared(ring);
 
@@ -404,6 +556,129 @@ __global__ void __launch_bounds__(ROW_THREADS, 2) attn_res_bwd2_k(ResBwd2Args A,
     issue();
   };
 
+  if constexpr (NCH > 8) {
+    // Wide rows: only dx_out stays in registers next to the assembled gradient g.  Every other item is read in place from its ring slot,
+    // once per pass (a hidden: the reductions, then c1 * h into accw); accw is a per-warp shared-memory row, the later layers' w are
+    // recomputed from gamma / pq per column group (L2-resident), and the c2 term of the newest hidden is applied with its own term, as its
+    // slot is refilled before the later layers' gradients arrive.
+    float* accw_s = w_s + D + (threadIdx.x >> 5) * D;
+    auto slot = [&]() { cp_async_wait<RING - 1>(); return ring + cons_slot * SLOT; };
+    auto release = [&]() { cons_slot = cons_slot + 1 == RING ? 0 : cons_slot + 1; issue(); };
+    if (A.own)
+      for (int c = threadIdx.x; c < D; c += ROW_THREADS) w_s[c] = (A.gam[0][c] + 1.f) * A.pq[0][c];
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) *reinterpret_cast<float4*>(accw_s + c * 128 + lane * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int i = 0; i < RING; ++i) issue();
+    __syncthreads();
+    for (int row = r0; row < r1; ++row) {
+      float g[NCH * 4];
+      const float4 scl = *reinterpret_cast<const float4*>(slot() + lane * 16);
+      release();
+      float c2sum = 0.f;
+      if (A.own) {
+        const float lse_r = __shfl_sync(0xffffffffu, scl.x, 31);
+        float dxv[NCH * 4];
+        take_f32(dxv);
+        float mean_da = 0.f;
+        {
+          const float* xs = reinterpret_cast<const float*>(slot());
+#pragma unroll
+          for (int c = 0; c < NCH; ++c) {
+            const float4 x4 = *reinterpret_cast<const float4*>(xs + c * 128 + lane * 4);
+            mean_da += x4.x * dxv[4 * c] + x4.y * dxv[4 * c + 1] + x4.z * dxv[4 * c + 2] + x4.w * dxv[4 * c + 3];
+          }
+          release();
+        }
+        mean_da = warp_sum(mean_da);
+        for (int k = 0; k < A.L1; ++k) {
+          const __nv_bfloat16* hs = reinterpret_cast<const __nv_bfloat16*>(slot()) + lane * 4;
+          float ss = 0.f, dot = 0.f, da = 0.f;
+#pragma unroll
+          for (int c = 0; c < NCH; ++c) {
+            const uint2 t = *reinterpret_cast<const uint2*>(hs + c * 128);
+            const float2 h01 = unpack2_bf16(t.x), h23 = unpack2_bf16(t.y);
+            const float4 w4 = *reinterpret_cast<const float4*>(w_s + c * 128 + lane * 4);
+            ss += h01.x * h01.x + h01.y * h01.y + h23.x * h23.x + h23.y * h23.y;
+            dot += h01.x * w4.x + h01.y * w4.y + h23.x * w4.z + h23.y * w4.w;
+            da += h01.x * dxv[4 * c] + h01.y * dxv[4 * c + 1] + h23.x * dxv[4 * c + 2] + h23.y * dxv[4 * c + 3];
+          }
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) {
+            ss += __shfl_xor_sync(0xffffffffu, ss, o); dot += __shfl_xor_sync(0xffffffffu, dot, o); da += __shfl_xor_sync(0xffffffffu, da, o);
+          }
+          const float nrm = fmaxf(sqrtf(ss), 1e-12f), rn = 1.f / nrm;
+          const float a = __expf(dot * rn - lse_r);
+          const float ds = a * (da - mean_da);
+          const float c1 = ds * rn, c2 = sqrtf(ss) < 1e-12f ? 0.f : ds * dot * rn * rn * rn;   // clamped norm: a constant for the gradient
+          const bool newest = k + 1 == A.L1;
+          if (newest) {
+            c2sum = c2;
+            for (int j = 0; j < A.n_later; ++j) c2sum += __shfl_sync(0xffffffffu, scl.z, j);
+          } else if (lane < 3) {
+            sc_out[(long long)row * sc_stride + k * 3 + lane] = lane == 0 ? a : (lane == 1 ? c1 : c2);
+          }
+#pragma unroll
+          for (int c = 0; c < NCH; ++c) {
+            const uint2 t = *reinterpret_cast<const uint2*>(hs + c * 128);
+            const float2 h01 = unpack2_bf16(t.x), h23 = unpack2_bf16(t.y);
+            float4* aw = reinterpret_cast<float4*>(accw_s + c * 128 + lane * 4);
+            float4 v = *aw;
+            v.x += c1 * h01.x; v.y += c1 * h01.y; v.z += c1 * h23.x; v.w += c1 * h23.y;
+            *aw = v;
+            if (newest) {                             // the newest hidden: its own term and the c2 term of every layer
+              const float4 w4 = *reinterpret_cast<const float4*>(w_s + c * 128 + lane * 4);
+              g[4 * c] = a * dxv[4 * c] + c1 * w4.x - c2sum * h01.x; g[4 * c + 1] = a * dxv[4 * c + 1] + c1 * w4.y - c2sum * h01.y;
+              g[4 * c + 2] = a * dxv[4 * c + 2] + c1 * w4.z - c2sum * h23.x; g[4 * c + 3] = a * dxv[4 * c + 3] + c1 * w4.w - c2sum * h23.y;
+            }
+          }
+          release();
+        }
+      } else {
+        for (int j = 0; j < A.n_later; ++j) c2sum += __shfl_sync(0xffffffffu, scl.z, j);
+        const __nv_bfloat16* hs = reinterpret_cast<const __nv_bfloat16*>(slot()) + lane * 4;
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) {
+          const uint2 t = *reinterpret_cast<const uint2*>(hs + c * 128);
+          const float2 h01 = unpack2_bf16(t.x), h23 = unpack2_bf16(t.y);
+          g[4 * c] = -c2sum * h01.x; g[4 * c + 1] = -c2sum * h01.y; g[4 * c + 2] = -c2sum * h23.x; g[4 * c + 3] = -c2sum * h23.y;
+        }
+        release();
+      }
+      for (int j = 0; j < A.n_later; ++j) {
+        const float* ds = reinterpret_cast<const float*>(slot()) + lane * 4;
+        const float a = __shfl_sync(0xffffffffu, scl.x, j), c1 = __shfl_sync(0xffffffffu, scl.y, j);
+        const float* gj = A.gam[j + 1] + lane * 4;
+        const float* pj = A.pq[j + 1] + lane * 4;
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) {
+          const float4 d4 = *reinterpret_cast<const float4*>(ds + c * 128);
+          const float4 ga = *reinterpret_cast<const float4*>(gj + c * 128), pa = *reinterpret_cast<const float4*>(pj + c * 128);
+          g[4 * c] += a * d4.x + c1 * ((ga.x + 1.f) * pa.x); g[4 * c + 1] += a * d4.y + c1 * ((ga.y + 1.f) * pa.y);
+          g[4 * c + 2] += a * d4.z + c1 * ((ga.z + 1.f) * pa.z); g[4 * c + 3] += a * d4.w + c1 * ((ga.w + 1.f) * pa.w);
+        }
+        release();
+      }
+      if (ACC) {
+        float o[NCH * 4];
+        load_row_f32<NCH>(G + (long long)row * D, lane, o);
+#pragma unroll
+        for (int i = 0; i < NCH * 4; ++i) g[i] += o[i];
+      }
+      store_row_f32<NCH>(G + (long long)row * D, lane, g);
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    if (A.own) {
+      __syncthreads();
+      for (int c = threadIdx.x; c < D; c += ROW_THREADS) {
+        float t = 0.f;
+#pragma unroll
+        for (int w = 0; w < WARPS_PER_BLOCK; ++w) t += w_s[D + w * D + c];
+        partials[(long long)blockIdx.x * D + c] = t;
+      }
+    }
+    return;
+  }
   for (int j = A.own ? 0 : 1; j <= A.n_later; ++j)
     for (int c = threadIdx.x; c < D; c += ROW_THREADS) w_s[j * D + c] = (A.gam[j][c] + 1.f) * A.pq[j][c];
 #pragma unroll
@@ -550,6 +825,64 @@ __global__ void __launch_bounds__(ROW_THREADS) rmsnorm_bwd_k(const float* __rest
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int r0 = warp * tpw, r1 = min(M, r0 + tpw);
   if (r0 >= M) return;
+  if constexpr (NCH > 8) {
+    // wide: passes for |x|, for <d xhat, xhat> and for the apply; d gamma accumulates in a per-warp shared-memory row (dynamic, 64 KB at 2048)
+    constexpr int W = WIDE_GROUP;
+    extern __shared__ __align__(16) float rms_acc[];
+    float* acc = rms_acc + (threadIdx.x >> 5) * D;
+    float t[W * 4];
+#pragma unroll
+    for (int i = 0; i < W * 4; ++i) t[i] = 0.f;
+#pragma unroll 1
+    for (int c0 = 0; c0 < NCH; c0 += W) store_row_f32<W>(acc + c0 * 128, lane, t);
+    const float c = sqrtf((float)D);
+    for (int row = r0; row < r1; ++row) {
+      const float* xr = x + (long long)row * D;
+      const float* dr = dout + (long long)row * D;
+      float ss = 0.f, dot = 0.f;
+#pragma unroll 1
+      for (int c0 = 0; c0 < NCH; c0 += W) {
+        load_row_f32<W>(xr + c0 * 128, lane, t);
+#pragma unroll
+        for (int i = 0; i < W * 4; ++i) ss += t[i] * t[i];
+      }
+      const float nrm = sqrtf(warp_sum(ss));
+      const float rn = 1.f / fmaxf(nrm, 1e-12f);
+#pragma unroll 1
+      for (int c0 = 0; c0 < NCH; c0 += W) {
+        float d[W * 4], gv[W * 4];
+        load_row_f32<W>(xr + c0 * 128, lane, t);
+        load_row_f32<W>(dr + c0 * 128, lane, d);
+        load_row_f32<W>(gamma + c0 * 128, lane, gv);
+#pragma unroll
+        for (int i = 0; i < W * 4; ++i) dot += d[i] * (c * (gv[i] + 1.f)) * (t[i] * rn);
+      }
+      dot = warp_sum(dot);
+      if (nrm < 1e-12f) dot = 0.f;
+#pragma unroll 1
+      for (int c0 = 0; c0 < NCH; c0 += W) {
+        float d[W * 4], gv[W * 4], a[W * 4];
+        load_row_f32<W>(xr + c0 * 128, lane, t);
+        load_row_f32<W>(dr + c0 * 128, lane, d);
+        load_row_f32<W>(gamma + c0 * 128, lane, gv);
+        load_row_f32<W>(acc + c0 * 128, lane, a);
+#pragma unroll
+        for (int i = 0; i < W * 4; ++i) {
+          t[i] *= rn;
+          a[i] += d[i] * t[i] * c;
+          d[i] = rn * (d[i] * (c * (gv[i] + 1.f)) - t[i] * dot);
+        }
+        store_row_f32<W>(acc + c0 * 128, lane, a);
+        store_row_f32<W>(dx + (long long)row * D + c0 * 128, lane, d);
+      }
+    }
+#pragma unroll 1
+    for (int c0 = 0; c0 < NCH; c0 += W) {
+      load_row_f32<W>(acc + c0 * 128, lane, t);
+      red_row_f32<W>(dgamma + c0 * 128, lane, t);
+    }
+    return;
+  }
   float gv[NCH * 4], acc[NCH * 4];
   load_row_f32<NCH>(gamma, lane, gv);
 #pragma unroll
@@ -904,7 +1237,7 @@ int tfx_adaln_fwd(const float* x, const int* cond_row, const float* film, long l
   if (M <= 0) return 0;
   TFX_DISPATCH_NCH(D, {
     auto kern = adaln_fwd_k<NCH>;
-    const int smem = WARPS_PER_BLOCK * ADALN_FWD_RING * D * 4;
+    const int smem = WARPS_PER_BLOCK * ADALN_FWD_RING<NCH> * D * 4;
     static int per_sm = 0;                            // persistent grid = the resident blocks (ring shared memory / registers decide)
     if (!per_sm) {
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -920,8 +1253,16 @@ int tfx_adaln_fwd(const float* x, const int* cond_row, const float* film, long l
 int tfx_adaln_bwd(const float* du, const float* x, const float* stats, const int* cond_row, const float* film, long long film_ld,
                   const float* ln_gamma, float* dx_accum, float* dfilm, long long dfilm_ld, float* dln_gamma, int M, int D, void* stream) {
   if (M <= 0) return 0;
-  const int tpw = balanced_tpw(M, num_sms(), 2, 4);
-  TFX_DISPATCH_NCH(D, (adaln_bwd_k<NCH><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(du, x, stats, cond_row, film, film_ld, ln_gamma, dx_accum, dfilm, dfilm_ld, dln_gamma, M, tpw)));
+  TFX_DISPATCH_NCH(D, {
+    // wide rows keep their accumulators in dynamic shared memory (3 rows per warp): one resident block per SM
+    const int smem = NCH > 8 ? WARPS_PER_BLOCK * 3 * D * 4 : 0;
+    if (NCH > 8) {
+      static bool attr_set = false;
+      if (!attr_set) { cudaFuncSetAttribute(adaln_bwd_k<NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr_set = true; }
+    }
+    const int tpw = balanced_tpw(M, num_sms(), NCH > 8 ? 1 : 2, 4);
+    adaln_bwd_k<NCH><<<chunk_grid(M, tpw), ROW_THREADS, smem, ST(stream)>>>(du, x, stats, cond_row, film, film_ld, ln_gamma, dx_accum, dfilm, dfilm_ld, dln_gamma, M, tpw);
+  });
   return check_launch("adaln_bwd");
 }
 
@@ -929,7 +1270,7 @@ int tfx_resid_bwd(const float* dx, const void* y_bf16, const int* cond_row, cons
                   void* dy_bf16, float* dzgate, long long dzgate_ld, float* dlayerscale, float* dbias, int M, int D, void* stream) {
   if (M <= 0) return 0;
   const int tpw = balanced_tpw(M, num_sms(), 2, 4);
-  const size_t smem = (dbias || layerscale) ? (size_t)WARPS_PER_BLOCK * D * sizeof(float) : 0;
+  const size_t smem = (dbias || layerscale) ? (size_t)WARPS_PER_BLOCK * (D > 1024 ? WIDE_GROUP * 128 : D) * sizeof(float) : 0;   // one column group
   TFX_DISPATCH_NCH(D, (resid_bwd_k<NCH><<<chunk_grid(M, tpw), ROW_THREADS, smem, ST(stream)>>>(dx, (const __nv_bfloat16*)y_bf16, cond_row, zgate, zgate_ld, layerscale,
                                                                                                  (__nv_bfloat16*)dy_bf16, dzgate, dzgate_ld, dlayerscale, dbias, M, tpw)));
   return check_launch("resid_bwd");
@@ -980,10 +1321,11 @@ int tfx_attn_residual_bwd2(const void* const* hiddens_bf16, int n_hiddens, int o
     for (int i = 0; i < n_hiddens; ++i) A.hid[i] = reinterpret_cast<const __nv_bfloat16*>(hiddens_bf16[i]);
     for (int j = 0; j <= n; ++j) { A.gam[j] = gammas[j0 + j]; A.pq[j] = pseudo_queries[j0 + j]; }
     for (int j = 0; j < n; ++j) { A.dx_later[j] = dx_later[j0 + j]; A.sc_later[j] = scalars_later[j0 + j]; }
-    const int slots = (1 + n) > WARPS_PER_BLOCK ? (1 + n) : WARPS_PER_BLOCK;
     TFX_DISPATCH_NCH(D, {
+      // w rows (wide: the own layer's w and the accw rows), then the rings
+      const int slots = NCH > 8 ? 1 + WARPS_PER_BLOCK : ((1 + n) > WARPS_PER_BLOCK ? (1 + n) : WARPS_PER_BLOCK);
       const size_t smem = (size_t)(slots + WARPS_PER_BLOCK * ResBwd2Cfg<NCH>::RING) * D * sizeof(float);
-      const int smem_max = (int)((BWD2_CHUNK + 1 + WARPS_PER_BLOCK * ResBwd2Cfg<NCH>::RING) * D * sizeof(float));
+      const int smem_max = (int)(((NCH > 8 ? 1 + WARPS_PER_BLOCK : BWD2_CHUNK + 1) + WARPS_PER_BLOCK * ResBwd2Cfg<NCH>::RING) * D * sizeof(float));
       static bool attr_set = false;               // (one flag per NCH instantiation; the size above is the maximum any call can ask for)
       if (!attr_set) {
         cudaFuncSetAttribute(attn_res_bwd2_k<NCH, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
@@ -1012,7 +1354,14 @@ int tfx_rmsnorm_fwd(const float* x, const float* gamma, float* out_f32, void* ou
 int tfx_rmsnorm_bwd(const float* dout, const float* x, const float* gamma, float* dx, float* dgamma, int M, int D, void* stream) {
   if (M <= 0) return 0;
   const int tpw = 16;
-  TFX_DISPATCH_NCH(D, (rmsnorm_bwd_k<NCH><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dout, x, gamma, dx, dgamma, M, tpw)));
+  TFX_DISPATCH_NCH(D, {
+    const int smem = NCH > 8 ? WARPS_PER_BLOCK * D * 4 : 0;      // wide rows: the d gamma accumulator rows
+    if (NCH > 8) {
+      static bool attr_set = false;
+      if (!attr_set) { cudaFuncSetAttribute(rmsnorm_bwd_k<NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr_set = true; }
+    }
+    rmsnorm_bwd_k<NCH><<<chunk_grid(M, tpw), ROW_THREADS, smem, ST(stream)>>>(dout, x, gamma, dx, dgamma, M, tpw);
+  });
   return check_launch("rmsnorm_bwd");
 }
 

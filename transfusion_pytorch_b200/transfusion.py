@@ -31,7 +31,7 @@ from .modality_processing import (
 # Deepest model the AttentionResidual kernels take (TFX_MAX_DEPTH in include/tfx_b200.h): their hidden-state lists hold x0 and 64 layer outputs
 MAX_DEPTH = 64
 # Model widths the row kernels are built for: the cases of TFX_DISPATCH_NCH (csrc/common.cuh), D = 128 * NCH
-MODEL_DIMS = (128, 256, 384, 512, 768, 1024)
+MODEL_DIMS = (128, 256, 384, 512, 768, 1024, 1536, 2048)
 # Heads the attention kernels take: two 64-wide heads per 128-column GEMM tile, at most 32 (gemm_qkvg's 32-column gate slab)
 MIN_HEADS, MAX_HEADS = 2, 32
 DIM_HEADS = (64, 128)                # attention head widths the kernels implement
