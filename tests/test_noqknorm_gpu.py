@@ -38,10 +38,10 @@ def Checks(what):
     return _Checks(what, SHOWN)
 
 
-def rope_tables(ops):
-    freqs = 1. / (10000 ** (torch.arange(0, 64, 2, device = 'cuda').float() / 64))
-    t = torch.empty(N_POS, 32, 2, device = 'cuda'); tt = torch.empty(32, N_POS, 2, device = 'cuda')
-    ops.rope_table(freqs, t, tt, N_POS, 32)
+def rope_tables(ops, dh = 64):
+    freqs = 1. / (10000 ** (torch.arange(0, dh, 2, device = 'cuda').float() / dh))
+    t = torch.empty(N_POS, dh // 2, 2, device = 'cuda'); tt = torch.empty(dh // 2, N_POS, 2, device = 'cuda')
+    ops.rope_table(freqs, t, tt, N_POS, dh // 2)
     return t, tt
 
 
@@ -54,49 +54,56 @@ def pair_sum(x):
     return (x[..., 0::2] + x[..., 1::2]).repeat_interleave(2, -1)
 
 
-def inputs(H, seed):
+def inputs(H, seed, dh = 64):
     D = DISPATCH_D[(H // 2) % len(DISPATCH_D)]
     g = gen(seed)
-    HI, NQ = 64 * H, 3 * 64 * H + 128
+    HI, NQ = dh * H, 3 * dh * H + 128
     u = torch.randn(M_ROWS, D, device = 'cuda', generator = g).to(BF16)
     W = (torch.randn(NQ, D, device = 'cuda', generator = g) / D ** 0.5).to(BF16)
-    gq, gk = (torch.rand(64, device = 'cuda', generator = g) * 1.9 - 0.9 for _ in range(2))
+    gq, gk = (torch.rand(dh, device = 'cuda', generator = g) * 1.9 - 0.9 for _ in range(2))
     pos = torch.randint(0, N_POS, (M_ROWS,), device = 'cuda', generator = g, dtype = I32)
     pos[::97] = N_POS - 1
-    return dict(D = D, H = H, HI = HI, NQ = NQ, mix = H <= 16, u = u, W = W, gq = gq, gk = gk, pos = pos)
+    return dict(D = D, H = H, dh = dh, HI = HI, NQ = NQ, mix = H <= 16, u = u, W = W, gq = gq, gk = gk, pos = pos)
 
 
 def run(ops, x, tt, rope_only, M = M_ROWS, kv = None):
+    """gemm_qkvg_rope or gemm_qkvg (their _d128 twins for 128-wide heads) into fresh guarded outputs"""
     H, HI, D = x['H'], x['HI'], x['D']
     out = {}
     for n, c, dt in (('q', HI, BF16), ('k', HI, BF16), ('v', HI, BF16), ('gates', H, F32), ('inv', 2 * H, F32), ('mix', H, F32)):
         out[n + '_buf'], out[n] = guarded(M, c, dt)
     k, v, rows = kv if kv is not None else (out['k'], out['v'], None)
     mix = out['mix'] if x['mix'] else None
-    if rope_only:
-        ops.gemm_qkvg_rope(x['u'], D, x['W'], D, M, H, D, out['q'], k, v, out['gates'], x['pos'], tt, N_POS, rows, mix)
+    rope_args = (x['u'], D, x['W'], D, M, H, D, out['q'], k, v, out['gates'], x['pos'], tt, N_POS, rows, mix)
+    norm_args = (x['u'], D, x['W'], D, M, H, D, out['q'], k, v, out['gates'], out['inv'], x['gq'], x['gk'], x['pos'], tt, N_POS, rows, mix)
+    if rope_only and x['dh'] == 128:
+        ops.gemm_qkvg_rope_d128(*rope_args)
+    elif rope_only:
+        ops.gemm_qkvg_rope(*rope_args)
+    elif x['dh'] == 128:
+        ops.gemm_qkvg_d128(*norm_args)
     else:
-        ops.gemm_qkvg(x['u'], D, x['W'], D, M, H, D, out['q'], k, v, out['gates'], out['inv'], x['gq'], x['gk'], x['pos'], tt, N_POS, rows, mix)
+        ops.gemm_qkvg(*norm_args)
     return out
 
 
 # ================================================================================================ kernels
 @pytest.mark.parametrize('H', HEADS)
-def test_gemm_qkvg_rope_vs_float64(ops, H):
-    x = inputs(H, seed = 500 + H)
+def test_gemm_qkvg_rope_vs_float64(ops, H, dh = 64):
+    x = inputs(H, seed = 500 + H, dh = dh)
     HI, M = x['HI'], M_ROWS
-    t, tt = rope_tables(ops)
+    t, tt = rope_tables(ops, dh)
     o = run(ops, x, tt, rope_only = True)
-    ck = Checks(f'qkvg_rope D={x["D"]} H={H}')
+    ck = Checks(f'qkvg_rope dh={dh} D={x["D"]} H={H}')
     a64, w64 = x['u'].double(), x['W'].double()
     y, mag = a64 @ w64.t(), a64.abs() @ w64.abs().t()
     cs = t[x['pos'].long()].double()
     c, s = cs[:, None, :, 0], cs[:, None, :, 1]
     for which, name in ((0, 'q'), (1, 'k')):
         sec = slice(which * HI, (which + 1) * HI)
-        ys, ms = y[:, sec].reshape(M, H, 64), mag[:, sec].reshape(M, H, 64)
+        ys, ms = y[:, sec].reshape(M, H, dh), mag[:, sec].reshape(M, H, dh)
         ref = rope64(ys, c, s)
-        ck(f'qkvg_rope {name}', o[name].reshape(M, H, 64), ref, U8 * ref.abs() + (1 + U8) * pair_sum(C_ACC * ms + 3 * U24 * ys.abs()))
+        ck(f'qkvg_rope {name}', o[name].reshape(M, H, dh), ref, U8 * ref.abs() + (1 + U8) * pair_sum(C_ACC * ms + 3 * U24 * ys.abs()))
     # v, gates and mix come from the same accumulators as gemm_qkvg's: identical bytes
     n = run(ops, x, tt, rope_only = False)
     for name in ('v', 'gates') + (('mix',) if x['mix'] else ()):
@@ -120,29 +127,36 @@ def test_gemm_qkvg_rope_vs_float64(ops, H):
 
 
 @pytest.mark.parametrize('H', HEADS)
-def test_qk_bwd_pack_rope_vs_float64(ops, H):
-    x = inputs(H, seed = 700 + H)
+def test_qk_bwd_pack_rope_vs_float64(ops, H, dh = 64):
+    x = inputs(H, seed = 700 + H, dh = dh)
     HI, NQ, M = x['HI'], x['NQ'], M_ROWS
-    t, tt = rope_tables(ops)
+    t, tt = rope_tables(ops, dh)
     o = run(ops, x, tt, rope_only = True)
     g = gen(800 + H)
     dq = torch.randn(M, HI, device = 'cuda', generator = g); dk = torch.randn(M, HI, device = 'cuda', generator = g)
     dsum = torch.randn(M, H, device = 'cuda', generator = g)
     out_buf, out = guarded(M, NQ, BF16)
-    ops.qk_bwd_pack_rope(dq, dk, x['pos'], t, o['gates'], dsum, out, NQ, M, H)
-    ck = Checks(f'qk_bwd_pack_rope H={H}')
+    if dh == 128:
+        ops.qk_bwd_pack_rope_d128(dq, dk, x['pos'], t, o['gates'], dsum, out, NQ, M, H)
+    else:
+        ops.qk_bwd_pack_rope(dq, dk, x['pos'], t, o['gates'], dsum, out, NQ, M, H)
+    ck = Checks(f'qk_bwd_pack_rope dh={dh} H={H}')
     cs = t[x['pos'].long()].double()
     c, s = cs[:, None, None, :, 0], cs[:, None, None, :, 1]
-    xx = torch.zeros(M, 2, H, 64, device = 'cuda', dtype = F64, requires_grad = True)
-    d64 = torch.stack((dq, dk), 1).double().reshape(M, 2, H, 64)
+    xx = torch.zeros(M, 2, H, dh, device = 'cuda', dtype = F64, requires_grad = True)
+    d64 = torch.stack((dq, dk), 1).double().reshape(M, 2, H, dh)
     (rope64(xx, c, s) * d64).sum().backward()
     ref = xx.grad
-    ck('qk_bwd_rope dx', out[:, :2 * HI].reshape(M, 2, H, 64), ref, U8 * ref.abs() + (1 + U8) * 3 * U24 * pair_sum(d64.abs()))
+    ck('qk_bwd_rope dx', out[:, :2 * HI].reshape(M, 2, H, dh), ref, U8 * ref.abs() + (1 + U8) * 3 * U24 * pair_sum(d64.abs()))
     # the gate column is qk_bwd_pack's, bit for bit
     n_buf, n = guarded(M, NQ, BF16)
     on = run(ops, x, tt, rope_only = False)
-    dgam = torch.zeros(2, 64, device = 'cuda')
-    ops.qk_bwd_pack(dq, dk, on['q'], on['k'], on['inv'], x['gq'], x['gk'], x['pos'], t, o['gates'], dsum, n, NQ, dgam[0], dgam[1], M, H)
+    dgam = torch.zeros(2, dh, device = 'cuda')
+    pack_args = (dq, dk, on['q'], on['k'], on['inv'], x['gq'], x['gk'], x['pos'], t, o['gates'], dsum, n, NQ, dgam[0], dgam[1], M, H)
+    if dh == 128:
+        ops.qk_bwd_pack_d128(*pack_args)
+    else:
+        ops.qk_bwd_pack(*pack_args)
     ck.true('gate column = qk_bwd_pack bytes', same_bits(out[:, 3 * HI:3 * HI + H], n[:, 3 * HI:3 * HI + H]))
     ck.true('dv columns untouched', untouched(out[:, 2 * HI:3 * HI]))
     ck.true('pad columns untouched', untouched(out[:, 3 * HI + H:]))
