@@ -61,12 +61,6 @@ __device__ __forceinline__ void load_tile(__nv_bfloat16* s, const __nv_bfloat16*
   }
 }
 
-// accurate tanh from two MUFU ops (ex2 + rcp): abs error ~1e-7, needed because the soft-cap multiplies it by 50
-__device__ __forceinline__ float tanh_acc(float x) {
-  const float e = __expf(2.f * x);
-  return 1.f - __fdividef(2.f, 1.f + e);
-}
-
 // ================================================================================================ forward
 // One CTA per (64-query tile, head), 4 warps of 16 query rows; K / V tiles double-buffered through cp.async.  The whole head is held in
 // registers (oacc DH / 2, qf DH / 4 per thread).
@@ -672,10 +666,8 @@ template <int DH>
 static int attn_bwd_prep(const char* name, const void* do_gated, const void* o_gated, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero,
                          int M, int H, void* stream) {
   if (M <= 0) return 0;
-  long long blocks = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  long long cap = (long long)num_sms() * 8;
-  attn_bwd_prep_k<DH><<<(int)(blocks < cap ? blocks : cap), ROW_THREADS, 0, ST(stream)>>>((const __nv_bfloat16*)do_gated, (const __nv_bfloat16*)o_gated, gates,
-                                                                                         (__nv_bfloat16*)do_pre, dsum_hm, dsum_mh, dq_zero, M, H);
+  attn_bwd_prep_k<DH><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>((const __nv_bfloat16*)do_gated, (const __nv_bfloat16*)o_gated, gates,
+                                                                            (__nv_bfloat16*)do_pre, dsum_hm, dsum_mh, dq_zero, M, H);
   return check_launch(name);
 }
 

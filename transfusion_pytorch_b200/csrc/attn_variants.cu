@@ -15,10 +15,6 @@ namespace tfx {
 
 int num_sms();
 
-__device__ __forceinline__ float tanh_acc_v(float x) {          // abs err ~1e-7 (same formulation as attention.cu)
-  const float e = __expf(2.f * x);
-  return 1.f - __fdividef(2.f, 1.f + e);
-}
 __device__ __forceinline__ float sigmoid_v(float x) { return 1.f / (1.f + __expf(-x)); }
 
 // One warp per token; DH / 8 lanes share a head (a lane owns 8 consecutive dims: 16-byte bf16 accesses), 32 / (DH / 8) heads per pass.
@@ -61,7 +57,7 @@ __global__ void __launch_bounds__(ROW_THREADS) laser_v_fwd_k(const __nv_bfloat16
     float x[8];
     ld8(v + r * ld_v + h * 64 + sub * 8, x);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) x[e] = __expf(c * tanh_acc_v(x[e] / c));
+    for (int e = 0; e < 8; ++e) x[e] = __expf(c * tanh_acc(x[e] / c));
     st8(vl + r * ld_vl + h * 64 + sub * 8, x);
   }
 }
@@ -75,7 +71,7 @@ __global__ void __launch_bounds__(ROW_THREADS) laser_v_bwd_k(__nv_bfloat16* __re
     ld8(dv + (long long)row * ld_dv + h * 64 + sub * 8, g);
     ld8(v + (long long)row * ld_v + h * 64 + sub * 8, x);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) { const float t = tanh_acc_v(x[e] / c); g[e] *= __expf(c * t) * (1.f - t * t); }
+    for (int e = 0; e < 8; ++e) { const float t = tanh_acc(x[e] / c); g[e] *= __expf(c * t) * (1.f - t * t); }
     st8(dv + (long long)row * ld_dv + h * 64 + sub * 8, g);
   }
 }
@@ -195,12 +191,6 @@ __global__ void __launch_bounds__(ROW_THREADS) add_f32_into_bf16_k(__nv_bfloat16
   }
 }
 
-static inline int row_grid(int M) {
-  long long blocks = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  long long cap = (long long)num_sms() * 8;
-  return (int)(blocks < cap ? (blocks < 1 ? 1 : blocks) : cap);
-}
-
 }  // namespace tfx
 
 using namespace tfx;
@@ -213,33 +203,33 @@ extern "C" {
 int tfx_laser_v_fwd(const void* v, long long ld_v, const int* rows, void* v_laser, long long ld_vl, int M, int H, float clamp, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(clamp > 0.f && ld_v % 8 == 0 && ld_vl % 8 == 0, "laser_v_fwd: clamp must be > 0 and row pitches multiples of 8 bf16");
-  laser_v_fwd_k<<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(v), ld_v, rows, BF(v_laser), ld_vl, M, H, clamp);
+  laser_v_fwd_k<<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(v), ld_v, rows, BF(v_laser), ld_vl, M, H, clamp);
   return check_launch("laser_v_fwd");
 }
 
 int tfx_laser_out_fwd(const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
   if (M <= 0) return 0;
-  laser_out_fwd_k<64><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
+  laser_out_fwd_k<64><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
   return check_launch("laser_out_fwd");
 }
 
 int tfx_laser_bwd_prep(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
   if (M <= 0) return 0;
-  laser_bwd_prep_k<64><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
+  laser_bwd_prep_k<64><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
   return check_launch("laser_bwd_prep");
 }
 
 int tfx_laser_v_bwd(void* dv_inout, long long ld_dv, const void* v, long long ld_v, int M, int H, float clamp, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(clamp > 0.f && ld_v % 8 == 0 && ld_dv % 8 == 0, "laser_v_bwd: clamp must be > 0 and row pitches multiples of 8 bf16");
-  laser_v_bwd_k<<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v), ld_v, M, H, clamp);
+  laser_v_bwd_k<<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v), ld_v, M, H, clamp);
   return check_launch("laser_v_bwd");
 }
 
 int tfx_vmix_fwd(void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias, int M, int H, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && mix_pre && mix_bias, "vmix_fwd: bad arguments");
-  vmix_fwd_k<64><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
+  vmix_fwd_k<64><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
   return check_launch("vmix_fwd");
 }
 
@@ -247,26 +237,26 @@ int tfx_vmix_bwd(void* dv_inout, long long ld_dv, const void* v_mixed, long long
                  float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && ld_dv % 8 == 0, "vmix_bwd: row pitches must be multiples of 8 bf16");
-  vmix_bwd_k<64><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc, BF(dmix_bf16), ld_dmix, M, H);
+  vmix_bwd_k<64><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc, BF(dmix_bf16), ld_dmix, M, H);
   return check_launch("vmix_bwd");
 }
 
 int tfx_laser_out_fwd_d128(const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
   if (M <= 0) return 0;
-  laser_out_fwd_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
+  laser_out_fwd_k<128><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
   return check_launch("laser_out_fwd_d128");
 }
 
 int tfx_laser_bwd_prep_d128(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
   if (M <= 0) return 0;
-  laser_bwd_prep_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
+  laser_bwd_prep_k<128><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
   return check_launch("laser_bwd_prep_d128");
 }
 
 int tfx_vmix_fwd_d128(void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias, int M, int H, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && mix_pre && mix_bias, "vmix_fwd_d128: bad arguments");
-  vmix_fwd_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
+  vmix_fwd_k<128><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
   return check_launch("vmix_fwd_d128");
 }
 
@@ -274,8 +264,8 @@ int tfx_vmix_bwd_d128(void* dv_inout, long long ld_dv, const void* v_mixed, long
                       float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && ld_dv % 8 == 0, "vmix_bwd_d128: row pitches must be multiples of 8 bf16");
-  vmix_bwd_k<128><<<row_grid(M), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc,
-                                                                 BF(dmix_bf16), ld_dmix, M, H);
+  vmix_bwd_k<128><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc,
+                                                                             BF(dmix_bf16), ld_dmix, M, H);
   return check_launch("vmix_bwd_d128");
 }
 

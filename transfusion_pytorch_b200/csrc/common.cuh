@@ -15,6 +15,19 @@ int check_launch(const char* what);     // cudaGetLastError -> 0 / negative code
 constexpr int WARPS_PER_BLOCK = 8;
 constexpr int ROW_THREADS = WARPS_PER_BLOCK * 32;
 
+// grid of the warp-per-row kernels (their warps stride over the rows): one warp per row, at most 8 blocks per SM
+inline int row_grid(int M, int sms) {
+  long long blocks = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
+  long long cap = (long long)sms * 8;
+  return (int)(blocks < cap ? (blocks < 1 ? 1 : blocks) : cap);
+}
+
+// accurate tanh from two MUFU ops (ex2 + rcp): abs error ~1e-7, needed because the attention soft-cap (50) and the LASER clamp (15) multiply it
+__device__ __forceinline__ float tanh_acc(float x) {
+  const float e = __expf(2.f * x);
+  return 1.f - __fdividef(2.f, 1.f + e);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -38,11 +38,6 @@ __global__ void decode_prep_k(const int* __restrict__ st, int S, int cap, int sl
   tq0[s] = s; tqend[s] = s + 1; tkv0[s] = base; tkvend[s] = base + len + 1;
 }
 
-__device__ __forceinline__ float tanh_acc_d(float x) {          // same formulation as attention.cu (abs err ~1e-7)
-  const float e = __expf(2.f * x);
-  return 1.f - __fdividef(2.f, 1.f + e);
-}
-
 // one CTA = one (single-query-row tile, head); 4 warps split the keys of the slab; lane <-> key for the scores, lane <-> 2 output dims for P V
 __global__ void __launch_bounds__(128) attn_decode_k(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k, const __nv_bfloat16* __restrict__ v,
                                                     long long ld_q, long long ld_k, long long ld_v, const float* __restrict__ gates, int H, const int* __restrict__ kv_limit,
@@ -74,7 +69,7 @@ __global__ void __launch_bounds__(128) attn_decode_k(const __nv_bfloat16* __rest
         d += x0.x * sq[c * 8] + x0.y * sq[c * 8 + 1] + x1.x * sq[c * 8 + 2] + x1.y * sq[c * 8 + 3] + x2.x * sq[c * 8 + 4] + x2.y * sq[c * 8 + 5] +
              x3.x * sq[c * 8 + 6] + x3.y * sq[c * 8 + 7];
       }
-      s = cap * tanh_acc_d(d * inv_cap);
+      s = cap * tanh_acc(d * inv_cap);
     }
     const float mn = fmaxf(m, warp_max(s));            // finite: lane 0 of this chunk is a valid key
     const float p = ok ? __expf(s - mn) : 0.f;
@@ -143,7 +138,7 @@ __global__ void __launch_bounds__(128) attn_decode_dh_k(const __nv_bfloat16* __r
         d += x0.x * sq[c * 8] + x0.y * sq[c * 8 + 1] + x1.x * sq[c * 8 + 2] + x1.y * sq[c * 8 + 3] + x2.x * sq[c * 8 + 4] + x2.y * sq[c * 8 + 5] +
              x3.x * sq[c * 8 + 6] + x3.y * sq[c * 8 + 7];
       }
-      s = cap * tanh_acc_d(d * inv_cap);
+      s = cap * tanh_acc(d * inv_cap);
     }
     const float mn = fmaxf(m, warp_max(s));            // finite: lane 0 of this chunk is a valid key
     const float p = ok ? __expf(s - mn) : 0.f;

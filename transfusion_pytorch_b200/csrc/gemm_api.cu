@@ -32,6 +32,29 @@ static int dispatch_major(const GemmOperand& A, const GemmOperand& B, const Gemm
   return launch_gemm_t<true, false, EPI_STORE>(A, B, p, sms, st);
 }
 
+// the four tfx_gemm_qkvg* entry points; `name` is the entry point's name for error messages.  W is [to_qk | to_v | to_gates | pad]
+// with N = 3 H DH + 128.  At DH = 64 a 128-column tile holds two heads, so H is even; at 128 it holds one, so any H in [1, 16].
+template <int EPI>
+static int gemm_qkvg(const char* name, const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v,
+                     float* gates, float* qk_inv, const float* q_gamma, const float* k_gamma, const int* rope_pos, const float* rope_cs_t, int rope_len,
+                     const int* kv_rows, float* mix_pre, void* stream) {
+  constexpr int DH = qkvg_dh(EPI);
+  if (M <= 0) return 0;
+  if constexpr (DH == 64) {
+    TFX_REQUIRE(!mix_pre || H <= 16, "%s: the value-residual mix columns share the 32-column gate slab: heads must be <= 16 (got %d)", name, H);
+    TFX_REQUIRE(H >= 2 && H % 2 == 0 && H <= 32, "%s: heads must be even and in [2, 32] (got %d)", name, H);
+  } else {
+    TFX_REQUIRE(H >= 1 && H <= 16, "%s: heads must be in [1, 16] (got %d)", name, H);
+  }
+  TFX_REQUIRE(ldu % 8 == 0 && ldw % 8 == 0, "%s: row pitches must be multiples of 8", name);
+  GemmParams p; memset(&p, 0, sizeof(p));
+  p.M = M; p.N = 3 * H * DH + 128; p.K = D; p.k_splits = 1; p.H = H;
+  p.q = (__nv_bfloat16*)q; p.k = (__nv_bfloat16*)k; p.v = (__nv_bfloat16*)v; p.gates = gates; p.qk_inv = qk_inv;
+  p.q_gamma = q_gamma; p.k_gamma = k_gamma; p.rope_pos = rope_pos; p.rope_cs = (const float2*)rope_cs_t; p.rope_len = rope_len; p.kv_rows = kv_rows; p.mix_pre = mix_pre;
+  GemmOperand a{u, ldu, false}, b{W, ldw, false};
+  return finish(launch_gemm_t<false, false, EPI>(a, b, p, num_sms(), ST(stream)), name);
+}
+
 extern "C" {
 
 int tfx_gemm_set_cluster_mode(int mode) {
@@ -76,57 +99,25 @@ int tfx_gemm_store(const void* A, long long lda, int a_mn_major, const void* B, 
 
 int tfx_gemm_qkvg(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates, float* qk_inv,
                   const float* q_gamma, const float* k_gamma, const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(!mix_pre || H <= 16, "gemm_qkvg: the value-residual mix columns share the 32-column gate slab: heads must be <= 16 (got %d)", H);
-  TFX_REQUIRE(H >= 2 && H % 2 == 0 && H <= 32, "gemm_qkvg: heads must be even and in [2, 32] (got %d)", H);
-  TFX_REQUIRE(ldu % 8 == 0 && ldw % 8 == 0, "gemm_qkvg: row pitches must be multiples of 8");
-  GemmParams p; memset(&p, 0, sizeof(p));
-  p.M = M; p.N = 3 * H * 64 + 128; p.K = D; p.k_splits = 1; p.H = H;
-  p.q = (__nv_bfloat16*)q; p.k = (__nv_bfloat16*)k; p.v = (__nv_bfloat16*)v; p.gates = gates; p.qk_inv = qk_inv;
-  p.q_gamma = q_gamma; p.k_gamma = k_gamma; p.rope_pos = rope_pos; p.rope_cs = (const float2*)rope_cs_t; p.rope_len = rope_len; p.kv_rows = kv_rows; p.mix_pre = mix_pre;
-  GemmOperand a{u, ldu, false}, b{W, ldw, false};
-  return finish(launch_gemm_t<false, false, EPI_QKVG>(a, b, p, num_sms(), ST(stream)), "gemm_qkvg");
+  return gemm_qkvg<EPI_QKVG>("gemm_qkvg", u, ldu, W, ldw, M, H, D, q, k, v, gates, qk_inv, q_gamma, k_gamma, rope_pos, rope_cs_t, rope_len, kv_rows, mix_pre, stream);
 }
 
 int tfx_gemm_qkvg_rope(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates,
                        const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(!mix_pre || H <= 16, "gemm_qkvg_rope: the value-residual mix columns share the 32-column gate slab: heads must be <= 16 (got %d)", H);
-  TFX_REQUIRE(H >= 2 && H % 2 == 0 && H <= 32, "gemm_qkvg_rope: heads must be even and in [2, 32] (got %d)", H);
-  TFX_REQUIRE(ldu % 8 == 0 && ldw % 8 == 0, "gemm_qkvg_rope: row pitches must be multiples of 8");
-  GemmParams p; memset(&p, 0, sizeof(p));
-  p.M = M; p.N = 3 * H * 64 + 128; p.K = D; p.k_splits = 1; p.H = H;
-  p.q = (__nv_bfloat16*)q; p.k = (__nv_bfloat16*)k; p.v = (__nv_bfloat16*)v; p.gates = gates;
-  p.rope_pos = rope_pos; p.rope_cs = (const float2*)rope_cs_t; p.rope_len = rope_len; p.kv_rows = kv_rows; p.mix_pre = mix_pre;
-  GemmOperand a{u, ldu, false}, b{W, ldw, false};
-  return finish(launch_gemm_t<false, false, EPI_QKVG_ROPE>(a, b, p, num_sms(), ST(stream)), "gemm_qkvg_rope");
+  return gemm_qkvg<EPI_QKVG_ROPE>("gemm_qkvg_rope", u, ldu, W, ldw, M, H, D, q, k, v, gates, nullptr, nullptr, nullptr, rope_pos, rope_cs_t, rope_len, kv_rows,
+                                  mix_pre, stream);
 }
 
-// head dim 128: W is [to_qk | to_v | to_gates | pad] with N = 3 H 128 + 128; one head per 128-column tile, so any H in [1, 16]
 int tfx_gemm_qkvg_d128(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates, float* qk_inv,
                        const float* q_gamma, const float* k_gamma, const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(H >= 1 && H <= 16, "gemm_qkvg_d128: heads must be in [1, 16] (got %d)", H);
-  TFX_REQUIRE(ldu % 8 == 0 && ldw % 8 == 0, "gemm_qkvg_d128: row pitches must be multiples of 8");
-  GemmParams p; memset(&p, 0, sizeof(p));
-  p.M = M; p.N = 3 * H * 128 + 128; p.K = D; p.k_splits = 1; p.H = H;
-  p.q = (__nv_bfloat16*)q; p.k = (__nv_bfloat16*)k; p.v = (__nv_bfloat16*)v; p.gates = gates; p.qk_inv = qk_inv;
-  p.q_gamma = q_gamma; p.k_gamma = k_gamma; p.rope_pos = rope_pos; p.rope_cs = (const float2*)rope_cs_t; p.rope_len = rope_len; p.kv_rows = kv_rows; p.mix_pre = mix_pre;
-  GemmOperand a{u, ldu, false}, b{W, ldw, false};
-  return finish(launch_gemm_t<false, false, EPI_QKVG_D128>(a, b, p, num_sms(), ST(stream)), "gemm_qkvg_d128");
+  return gemm_qkvg<EPI_QKVG_D128>("gemm_qkvg_d128", u, ldu, W, ldw, M, H, D, q, k, v, gates, qk_inv, q_gamma, k_gamma, rope_pos, rope_cs_t, rope_len, kv_rows,
+                                  mix_pre, stream);
 }
 
 int tfx_gemm_qkvg_rope_d128(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates,
                             const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(H >= 1 && H <= 16, "gemm_qkvg_rope_d128: heads must be in [1, 16] (got %d)", H);
-  TFX_REQUIRE(ldu % 8 == 0 && ldw % 8 == 0, "gemm_qkvg_rope_d128: row pitches must be multiples of 8");
-  GemmParams p; memset(&p, 0, sizeof(p));
-  p.M = M; p.N = 3 * H * 128 + 128; p.K = D; p.k_splits = 1; p.H = H;
-  p.q = (__nv_bfloat16*)q; p.k = (__nv_bfloat16*)k; p.v = (__nv_bfloat16*)v; p.gates = gates;
-  p.rope_pos = rope_pos; p.rope_cs = (const float2*)rope_cs_t; p.rope_len = rope_len; p.kv_rows = kv_rows; p.mix_pre = mix_pre;
-  GemmOperand a{u, ldu, false}, b{W, ldw, false};
-  return finish(launch_gemm_t<false, false, EPI_QKVG_ROPE_D128>(a, b, p, num_sms(), ST(stream)), "gemm_qkvg_rope_d128");
+  return gemm_qkvg<EPI_QKVG_ROPE_D128>("gemm_qkvg_rope_d128", u, ldu, W, ldw, M, H, D, q, k, v, gates, nullptr, nullptr, nullptr, rope_pos, rope_cs_t, rope_len,
+                                       kv_rows, mix_pre, stream);
 }
 
 int tfx_gemm_resid(const void* A, long long lda, const void* A2, long long lda2, int K1, const void* W, long long ldw, int M, int N, int K, const float* bias,

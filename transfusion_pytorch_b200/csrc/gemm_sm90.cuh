@@ -42,6 +42,10 @@ constexpr int GEMM_UK = 16;     // wgmma K for 16-bit inputs
 // GEGLU_DROP: GEGLU with FFN dropout on h.  QKVG_ROPE: QKVG without the qk-RMSNorm (`qk_rmsnorm = False`): q, k = RoPE(acc), no qk_inv
 // QKVG_D128 / QKVG_ROPE_D128: QKVG / QKVG_ROPE at head dim 128 (one head per 128-column tile; rope_cs is [64][rope_len])
 enum : int { EPI_STORE = 0, EPI_QKVG = 1, EPI_RESID = 2, EPI_GEGLU = 3, EPI_GEGLU_DROP = 4, EPI_QKVG_ROPE = 5, EPI_QKVG_D128 = 6, EPI_QKVG_ROPE_D128 = 7 };
+// the four QKVG epilogues are one body: head width (64 or 128) and whether q / k get the qk-RMSNorm
+constexpr bool epi_is_qkvg(int e) { return e == EPI_QKVG || e == EPI_QKVG_ROPE || e == EPI_QKVG_D128 || e == EPI_QKVG_ROPE_D128; }
+constexpr int qkvg_dh(int e) { return e == EPI_QKVG_D128 || e == EPI_QKVG_ROPE_D128 ? 128 : 64; }
+constexpr bool qkvg_norm(int e) { return e == EPI_QKVG || e == EPI_QKVG_D128; }
 
 struct GemmParams {
   int M, N, K;                 // D is M x N, reduction K
@@ -54,15 +58,16 @@ struct GemmParams {
   float alpha;
   int accumulate_f32;          // 1: out_f32 += (red.add)
   int K1;                      // A is the concatenation [A | A2] along K; A2 starts at k = K1 (K1 % 64 == 0); K1 = K when unused
-  // ---- EPI_QKVG (N tile 128 = 2 heads: H/2 q tiles | H/2 k tiles | H/2 v tiles | 1 gate tile)
-  int H;                       // heads (even), head dim 64
-  __nv_bfloat16 *q, *k, *v;    // [M][H*64]
+  // ---- EPI_QKVG* at head dim DH = 64 or 128 (N tile 128 = 128 / DH heads: H DH / 128 q tiles | as many k | as many v | 1 gate tile)
+  int H;                       // heads (even at DH = 64)
+  __nv_bfloat16 *q, *k, *v;    // [M][H*DH]
   float* gates;                // [M][H]   raw gate logits
-  float* mix_pre;              // [M][H]   optional: columns [H, 2H) of the gate tile = pre-activation of the learned value-residual mix (T.py:956-960)
+  float* mix_pre;              // [M][H]   optional: columns [m0, m0 + H) of the gate tile, m0 = H rounded up to even, = pre-activation of the
+                               //          learned value-residual mix (T.py:956-960)
   float* qk_inv;               // [M][2H]  1/max(|x|,eps) for q heads then k heads
-  const float *q_gamma, *k_gamma;   // [64]
+  const float *q_gamma, *k_gamma;   // [DH]
   const int* rope_pos;         // [M]
-  const float2* rope_cs;       // [32][rope_len] (cos, sin): transposed table, consecutive positions are contiguous
+  const float2* rope_cs;       // [DH/2][rope_len] (cos, sin): transposed table, consecutive positions are contiguous
   int rope_len;
   const int* kv_rows;          // optional [M]: destination ROW of token m inside k / v (in-place kv-cache append: k, v then point at a
                                // layer's cache slabs and q stays dense); null = row m
@@ -450,6 +455,7 @@ __global__ void __launch_bounds__(384, 1)
 gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using Cfg = GemmCfg<EPI>;
   constexpr bool GEGLU = EPI == EPI_GEGLU || EPI == EPI_GEGLU_DROP;
+  constexpr bool QKVG = epi_is_qkvg(EPI);
   constexpr int BN = GEMM_BN;
   constexpr int STAGES = Cfg::STAGES;
   static_assert(Cfg::STAGE_BYTES % 1024 == 0 && 2 * STAGES <= 32, "stage alignment / barrier area");
@@ -546,7 +552,7 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int rows_valid = min(32, p.M - wrow0);            // may be <= 0
       const int col0 = n_blk * BN;
       int qk_pos = 0;
-      if constexpr (EPI == EPI_QKVG || EPI == EPI_QKVG_ROPE || EPI == EPI_QKVG_D128 || EPI == EPI_QKVG_ROPE_D128) { qk_pos = row_ok ? p.rope_pos[row] : 0; }
+      if constexpr (QKVG) { qk_pos = row_ok ? p.rope_pos[row] : 0; }
       if constexpr (EPI == EPI_RESID) { qk_pos = (row_ok && p.cond_row) ? p.cond_row[row] : -1; }      // (reused as the condition row)
 
       if constexpr (EPI == EPI_STORE) {
@@ -558,95 +564,29 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           acc_ld32(acc, erow, c * 32, r);
           store_slice(p, sw, lane, r, cbase, [&](int i) { return wrow0 + i; });
         }
-      } else if constexpr (EPI == EPI_QKVG || EPI == EPI_QKVG_ROPE) {
-        const int tps = p.H >> 1;             // tiles per section
+      } else if constexpr (QKVG) {
+        // N tiles: H DH / 128 q tiles | as many k tiles | as many v tiles | 1 gate tile; a tile holds 128 / DH heads
+        constexpr int DH = qkvg_dh(EPI), HPT = BN / DH;
+        constexpr float SQRT_DH = DH == 64 ? 8.f : 11.313708498984761f;
+        const int tps = (p.H * DH) >> 7;      // tiles per section, H DH / 128 (H > 0: a shift, where a signed divide costs instructions)
         const int kind = n_blk / tps;         // 0 q, 1 k, 2 v, 3 gates
         const int tis = n_blk - kind * tps;   // tile in section
-        const long long HI = (long long)p.H * 64;
+        const long long HI = (long long)p.H * DH;
         if (kind <= 1) {
           const float* gamma = kind == 0 ? p.q_gamma : p.k_gamma;
           __nv_bfloat16* dstm = kind == 0 ? p.q : p.k;
           const float2* cs = p.rope_cs + qk_pos;        // entry i of this row's position: cs[i * rope_len]
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {              // the tile's two heads
-            uint32_t r0[32], r1[32];
-            acc_ld32(acc, erow, hh * 64, r0);
-            acc_ld32(acc, erow, hh * 64 + 32, r1);
-            float sc = 1.f;                               // qk-RMSNorm: 8 / |x| (times gamma + 1 per dim below)
-            if constexpr (EPI == EPI_QKVG) {
-              float ss = 0.f;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) { float a = __uint_as_float(r0[j]), b = __uint_as_float(r1[j]); ss += a * a + b * b; }
-              const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
-              if (row_ok) p.qk_inv[(long long)row * 2 * p.H + kind * p.H + tis * 2 + hh] = inv;
-              sc = inv * 8.f;
-            }
-            const int head = tis * 2 + hh;
-            uint32_t outw[32];
-#pragma unroll
-            for (int dh = 0; dh < 2; ++dh) {              // the head's two 32-dim halves
-              uint32_t* rr = dh == 0 ? r0 : r1;
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const int d0 = dh * 32 + 2 * i;
-                float y0 = __uint_as_float(rr[2 * i]), y1 = __uint_as_float(rr[2 * i + 1]);
-                if constexpr (EPI == EPI_QKVG) {
-                  const float2 gm = *reinterpret_cast<const float2*>(gamma + d0);
-                  y0 = y0 * sc * (gm.x + 1.f);
-                  y1 = y1 * sc * (gm.y + 1.f);
-                }
-                const float2 cc = cs[(long long)(dh * 16 + i) * p.rope_len];
-                outw[dh * 16 + i] = pack_bf16(y0 * cc.x - y1 * cc.y, y1 * cc.x + y0 * cc.y);
-              }
-            }
-            stg_put<8>(sw, lane, outw);
-            __syncwarp();
-            if (kind == 1 && p.kv_rows) stg_store_rows<8>(sw, lane, reinterpret_cast<uint8_t*>(dstm + head * 64), HI * 2, rows_valid, p.kv_rows + wrow0);
-            else stg_store<8>(sw, lane, reinterpret_cast<uint8_t*>(dstm + (long long)wrow0 * HI + head * 64), HI * 2, rows_valid);
-            __syncwarp();
-          }
-        } else if (kind == 2) {
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t r0[32], r1[32], w[32];
-            acc_ld32(acc, erow, c * 64, r0);
-            acc_ld32(acc, erow, c * 64 + 32, r1);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              w[j] = pack_bf16(__uint_as_float(r0[2 * j]), __uint_as_float(r0[2 * j + 1]));
-              w[16 + j] = pack_bf16(__uint_as_float(r1[2 * j]), __uint_as_float(r1[2 * j + 1]));
-            }
-            stg_put<8>(sw, lane, w);
-            __syncwarp();
-            if (p.kv_rows) stg_store_rows<8>(sw, lane, reinterpret_cast<uint8_t*>(p.v + tis * 128 + c * 64), HI * 2, rows_valid, p.kv_rows + wrow0);
-            else stg_store<8>(sw, lane, reinterpret_cast<uint8_t*>(p.v + (long long)wrow0 * HI + tis * 128 + c * 64), HI * 2, rows_valid);
-            __syncwarp();
-          }
-        } else {
-          uint32_t r[32];
-          acc_ld32(acc, erow, 0, r);
-          if (row_ok) {
-            float* dst = p.gates + (long long)row * p.H;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) if (j < p.H) dst[j] = __uint_as_float(r[j]);
-            if (p.mix_pre) {
-              float* dm = p.mix_pre + (long long)row * p.H;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) if (j >= p.H && j < 2 * p.H) dm[j - p.H] = __uint_as_float(r[j]);
-            }
-          }
-        }
-      } else if constexpr (EPI == EPI_QKVG_D128 || EPI == EPI_QKVG_ROPE_D128) {
-        // head dim 128: N tile = 1 head (H q tiles | H k tiles | H v tiles | 1 gate tile); the q / k norm spans the whole tile row
-        const int kind = n_blk / p.H;         // 0 q, 1 k, 2 v, 3 gates
-        const int tis = n_blk - kind * p.H;   // tile in section = head
-        const long long HI = (long long)p.H * 128;
-        if (kind <= 1) {
-          const float* gamma = kind == 0 ? p.q_gamma : p.k_gamma;
-          __nv_bfloat16* dstm = kind == 0 ? p.q : p.k;
-          const float2* cs = p.rope_cs + qk_pos;        // entry i of this row's position: cs[i * rope_len]
-          float sc = 1.f;                               // qk-RMSNorm: sqrt(128) / |x| (times gamma + 1 per dim below)
-          if constexpr (EPI == EPI_QKVG_D128) {
+          // qk-RMSNorm of the head that starts in the tile's 64-column half hh, from its sum of squares: 1/|x| goes to qk_inv, and the
+          // columns are scaled by sqrt(DH) / |x| (times gamma + 1 per column below).  The sum is taken where each width has its head:
+          // at 128 the whole tile row, re-read from shared memory before the halves so that 128 accumulators are not held in registers;
+          // at 64 the two slices of the half just loaded.
+          float sc = 1.f;
+          auto norm = [&](float ss, int hh) {
+            const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
+            if (row_ok) p.qk_inv[(long long)row * 2 * p.H + kind * p.H + tis * HPT + hh * 64 / DH] = inv;
+            sc = inv * SQRT_DH;
+          };
+          if constexpr (qkvg_norm(EPI) && DH == 128) {
             float ss = 0.f;
 #pragma unroll 1
             for (int c = 0; c < 4; ++c) {
@@ -655,24 +595,30 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
               for (int j = 0; j < 32; ++j) { const float a = __uint_as_float(r[j]); ss += a * a; }
             }
-            const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
-            if (row_ok) p.qk_inv[(long long)row * 2 * p.H + kind * p.H + tis] = inv;
-            sc = inv * 11.313708498984761f;
+            norm(ss, 0);
           }
 #pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {              // the head's two 64-column halves
+          for (int hh = 0; hh < 2; ++hh) {              // the tile's two 64-column halves
+            const int c0 = hh * 64 % DH;                  // the half's first column within its head
             uint32_t r0[32], r1[32];
             acc_ld32(acc, erow, hh * 64, r0);
             acc_ld32(acc, erow, hh * 64 + 32, r1);
+            if constexpr (qkvg_norm(EPI) && DH == 64) {
+              float ss = 0.f;
+#pragma unroll
+              for (int j = 0; j < 32; ++j) { float a = __uint_as_float(r0[j]), b = __uint_as_float(r1[j]); ss += a * a + b * b; }
+              norm(ss, hh);
+            }
+            const int head = tis * HPT + hh * 64 / DH;
             uint32_t outw[32];
 #pragma unroll
-            for (int dh = 0; dh < 2; ++dh) {
+            for (int dh = 0; dh < 2; ++dh) {              // the half's two 32-column slices
               uint32_t* rr = dh == 0 ? r0 : r1;
 #pragma unroll
               for (int i = 0; i < 16; ++i) {
-                const int d0 = hh * 64 + dh * 32 + 2 * i;
+                const int d0 = c0 + dh * 32 + 2 * i;     // column within the head
                 float y0 = __uint_as_float(rr[2 * i]), y1 = __uint_as_float(rr[2 * i + 1]);
-                if constexpr (EPI == EPI_QKVG_D128) {
+                if constexpr (qkvg_norm(EPI)) {
                   const float2 gm = *reinterpret_cast<const float2*>(gamma + d0);
                   y0 = y0 * sc * (gm.x + 1.f);
                   y1 = y1 * sc * (gm.y + 1.f);
@@ -683,8 +629,8 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
             stg_put<8>(sw, lane, outw);
             __syncwarp();
-            if (kind == 1 && p.kv_rows) stg_store_rows<8>(sw, lane, reinterpret_cast<uint8_t*>(dstm + tis * 128 + hh * 64), HI * 2, rows_valid, p.kv_rows + wrow0);
-            else stg_store<8>(sw, lane, reinterpret_cast<uint8_t*>(dstm + (long long)wrow0 * HI + tis * 128 + hh * 64), HI * 2, rows_valid);
+            if (kind == 1 && p.kv_rows) stg_store_rows<8>(sw, lane, reinterpret_cast<uint8_t*>(dstm + head * DH + c0), HI * 2, rows_valid, p.kv_rows + wrow0);
+            else stg_store<8>(sw, lane, reinterpret_cast<uint8_t*>(dstm + (long long)wrow0 * HI + head * DH + c0), HI * 2, rows_valid);
             __syncwarp();
           }
         } else if (kind == 2) {
@@ -708,14 +654,20 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           uint32_t r[32];
           acc_ld32(acc, erow, 0, r);
           if (row_ok) {
+            constexpr int H_MAX = DH == 64 ? 32 : 16;   // the largest head count the entry points accept at this width
             float* dst = p.gates + (long long)row * p.H;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) if (j < p.H) dst[j] = __uint_as_float(r[j]);
+            for (int j = 0; j < H_MAX; ++j) if (j < p.H) dst[j] = __uint_as_float(r[j]);
             if (p.mix_pre) {                            // mix columns start at an even column (bf16 pairs of their gradient stay 4-byte aligned)
               const int m0 = (p.H + 1) & ~1;
               float* dm = p.mix_pre + (long long)row * p.H;
 #pragma unroll
-              for (int j = 0; j < 32; ++j) if (j >= m0 && j < m0 + p.H) dm[j - m0] = __uint_as_float(r[j]);
+              for (int j = 0; j < 32; ++j) {
+                // H is even at width 64, so the start is H.  Spelled per width so that each keeps its generated code: p.H read per
+                // column at 64, the rounded start computed once at 128.
+                const int mj = DH == 64 ? p.H : m0;
+                if (j >= mj && j < mj + p.H) dm[j - mj] = __uint_as_float(r[j]);
+              }
             }
           }
         }

@@ -1207,12 +1207,6 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_rope_k(const float* _
   }
 }
 
-int num_sms();
-static inline int row_grid(int M, int sms) {
-  long long blocks = ((long long)M + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK;
-  long long cap = (long long)sms * 8;
-  return (int)(blocks < cap ? (blocks < 1 ? 1 : blocks) : cap);
-}
 // rows per warp such that the grid is (just under) one full wave of `blocks_per_sm` resident blocks on every SM
 static inline int balanced_tpw(int M, int sms, int blocks_per_sm, int min_tpw) {
   const long long warps = (long long)sms * blocks_per_sm * WARPS_PER_BLOCK;
