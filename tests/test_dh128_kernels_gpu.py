@@ -6,10 +6,11 @@ width; same layouts, invariants, sentinels and bound definitions):
   inside the qk-RMSNorm range (|s / cap| ~ 0.7 from planted q = +-k rows), at gamma = 0, and unnormalised (|s / cap| > 3, the soft cap
   saturated); per-(token, head) row errors against the magnitudes of the summed terms; dv into the packed dqkvg matrix between sentinels,
   dq / dk pre-filled.  Keys and queries that cannot see each other change nothing, bit for bit (64-key backward tiles); cached prefill from
-  a slab cache; the LASER / value-residual chain in engine order, and its row kernels one by one.
+  a slab cache; the LASER / value-residual chain in engine order, and its row kernels one by one (laser_out_fwd_k<128>,
+  laser_bwd_prep_k<128>, vmix_fwd_k<128>, vmix_bwd_k<128>).
 - decode.cu's attn_decode_dh_k<128>: every fill length, out-of-order slabs, NaN past the visible keys, padded pitches, saturated and LASER.
 - the QKVG d128 epilogues (qk-RMSNorm and RoPE-only) in both GEMM cluster modes, with and without the mix rows, the kv-cache append of prefill
-  and of a decode step, guard rows; qk_bwd_pack_d128 / _rope_d128.
+  and of a decode step, guard rows; qk_bwd_pack_d128 / _rope_d128 (qk_bwd_pack_k<128, true> / <128, false>).
 
 Bounds: the attention bounds are TOL_D128 in tests/test_attention_layer_gpu.py (about 3x the worst error measured over this file, measured
 value beside each); the decode and GEMM-epilogue bounds are the first-principles bounds of their 64-wide tests with the head width put in.

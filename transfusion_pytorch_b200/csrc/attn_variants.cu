@@ -198,6 +198,41 @@ using namespace tfx;
 #define BF(p) reinterpret_cast<__nv_bfloat16*>(p)
 #define CBF(p) reinterpret_cast<const __nv_bfloat16*>(p)
 
+// launchers of the per-head kernels, behind each entry point and its _d128 twin; `name` is the entry point's name for error messages
+template <int DH>
+static int laser_out_fwd(const char* name, const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  laser_out_fwd_k<DH><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
+  return check_launch(name);
+}
+
+template <int DH>
+static int laser_bwd_prep(const char* name, const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero,
+                          int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  laser_bwd_prep_k<DH><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
+  return check_launch(name);
+}
+
+template <int DH>
+static int vmix_fwd(const char* name, void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre,
+                    const float* mix_bias, int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && mix_pre && mix_bias, "%s: bad arguments", name);
+  vmix_fwd_k<DH><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
+  return check_launch(name);
+}
+
+template <int DH>
+static int vmix_bwd(const char* name, void* dv_inout, long long ld_dv, const void* v_mixed, long long ld_v, const void* v_first, long long ld_v0,
+                    const float* mix_pre, const float* mix_bias, float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && ld_dv % 8 == 0, "%s: row pitches must be multiples of 8 bf16", name);
+  vmix_bwd_k<DH><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc,
+                                                                         BF(dmix_bf16), ld_dmix, M, H);
+  return check_launch(name);
+}
+
 extern "C" {
 
 int tfx_laser_v_fwd(const void* v, long long ld_v, const int* rows, void* v_laser, long long ld_vl, int M, int H, float clamp, void* stream) {
@@ -207,18 +242,6 @@ int tfx_laser_v_fwd(const void* v, long long ld_v, const int* rows, void* v_lase
   return check_launch("laser_v_fwd");
 }
 
-int tfx_laser_out_fwd(const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  laser_out_fwd_k<64><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
-  return check_launch("laser_out_fwd");
-}
-
-int tfx_laser_bwd_prep(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  laser_bwd_prep_k<64><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
-  return check_launch("laser_bwd_prep");
-}
-
 int tfx_laser_v_bwd(void* dv_inout, long long ld_dv, const void* v, long long ld_v, int M, int H, float clamp, void* stream) {
   if (M <= 0) return 0;
   TFX_REQUIRE(clamp > 0.f && ld_v % 8 == 0 && ld_dv % 8 == 0, "laser_v_bwd: clamp must be > 0 and row pitches multiples of 8 bf16");
@@ -226,47 +249,38 @@ int tfx_laser_v_bwd(void* dv_inout, long long ld_dv, const void* v, long long ld
   return check_launch("laser_v_bwd");
 }
 
+int tfx_laser_out_fwd(const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
+  return laser_out_fwd<64>("laser_out_fwd", o_laser, gates, att, M, H, stream);
+}
+
+int tfx_laser_out_fwd_d128(const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
+  return laser_out_fwd<128>("laser_out_fwd_d128", o_laser, gates, att, M, H, stream);
+}
+
+int tfx_laser_bwd_prep(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
+  return laser_bwd_prep<64>("laser_bwd_prep", d_att, o_laser, gates, do_pre, dsum_hm, dsum_mh, dq_zero, M, H, stream);
+}
+
+int tfx_laser_bwd_prep_d128(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
+  return laser_bwd_prep<128>("laser_bwd_prep_d128", d_att, o_laser, gates, do_pre, dsum_hm, dsum_mh, dq_zero, M, H, stream);
+}
+
 int tfx_vmix_fwd(void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && mix_pre && mix_bias, "vmix_fwd: bad arguments");
-  vmix_fwd_k<64><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
-  return check_launch("vmix_fwd");
+  return vmix_fwd<64>("vmix_fwd", v_inout, ld_v, rows, v_first, ld_v0, mix_pre, mix_bias, M, H, stream);
+}
+
+int tfx_vmix_fwd_d128(void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias, int M, int H, void* stream) {
+  return vmix_fwd<128>("vmix_fwd_d128", v_inout, ld_v, rows, v_first, ld_v0, mix_pre, mix_bias, M, H, stream);
 }
 
 int tfx_vmix_bwd(void* dv_inout, long long ld_dv, const void* v_mixed, long long ld_v, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias,
                  float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && ld_dv % 8 == 0, "vmix_bwd: row pitches must be multiples of 8 bf16");
-  vmix_bwd_k<64><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc, BF(dmix_bf16), ld_dmix, M, H);
-  return check_launch("vmix_bwd");
-}
-
-int tfx_laser_out_fwd_d128(const void* o_laser, const float* gates, void* att, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  laser_out_fwd_k<128><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(o_laser), gates, BF(att), M, H);
-  return check_launch("laser_out_fwd_d128");
-}
-
-int tfx_laser_bwd_prep_d128(const void* d_att, const void* o_laser, const float* gates, void* do_pre, float* dsum_hm, float* dsum_mh, float* dq_zero, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  laser_bwd_prep_k<128><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(CBF(d_att), CBF(o_laser), gates, BF(do_pre), dsum_hm, dsum_mh, dq_zero, M, H);
-  return check_launch("laser_bwd_prep_d128");
-}
-
-int tfx_vmix_fwd_d128(void* v_inout, long long ld_v, const int* rows, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && mix_pre && mix_bias, "vmix_fwd_d128: bad arguments");
-  vmix_fwd_k<128><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(v_inout), ld_v, rows, CBF(v_first), ld_v0, mix_pre, mix_bias, M, H);
-  return check_launch("vmix_fwd_d128");
+  return vmix_bwd<64>("vmix_bwd", dv_inout, ld_dv, v_mixed, ld_v, v_first, ld_v0, mix_pre, mix_bias, dv_first_acc, dmix_bf16, ld_dmix, M, H, stream);
 }
 
 int tfx_vmix_bwd_d128(void* dv_inout, long long ld_dv, const void* v_mixed, long long ld_v, const void* v_first, long long ld_v0, const float* mix_pre, const float* mix_bias,
                       float* dv_first_acc, void* dmix_bf16, long long ld_dmix, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(ld_v % 8 == 0 && ld_v0 % 8 == 0 && ld_dv % 8 == 0, "vmix_bwd_d128: row pitches must be multiples of 8 bf16");
-  vmix_bwd_k<128><<<row_grid(M, num_sms()), ROW_THREADS, 0, ST(stream)>>>(BF(dv_inout), ld_dv, CBF(v_mixed), ld_v, CBF(v_first), ld_v0, mix_pre, mix_bias, dv_first_acc,
-                                                                             BF(dmix_bf16), ld_dmix, M, H);
-  return check_launch("vmix_bwd_d128");
+  return vmix_bwd<128>("vmix_bwd_d128", dv_inout, ld_dv, v_mixed, ld_v, v_first, ld_v0, mix_pre, mix_bias, dv_first_acc, dmix_bf16, ld_dmix, M, H, stream);
 }
 
 int tfx_add_f32_into_bf16(void* dst_bf16, long long ld_dst, const float* src, long long ld_src, int M, int N, void* stream) {

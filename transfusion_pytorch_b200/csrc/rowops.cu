@@ -1059,14 +1059,15 @@ __global__ void __launch_bounds__(ROW_THREADS) clean_flow_bwd_k(float* __restric
 }
 
 // ------------------------------------------------------------------------------------ qk RMSNorm + RoPE backward, packs d[q|k|.|gates]
-// forward (GEMM epilogue): xhat = x*inv;  y = xhat*sqrt(DH)*(gamma+1);  q = R(pos) y (interleaved pairs)   (T.py:950-965)
+// NORM (qk_rmsnorm = True), forward in the GEMM epilogue: xhat = x*inv;  y = xhat*sqrt(DH)*(gamma+1);  q = R(pos) y (interleaved pairs)
+// (T.py:950-965).  !NORM (EPI_QKVG_ROPE): q = R(pos) x, so d x = R(pos)^T d q per interleaved pair; no saved values and no gammas are needed.
 // One warp per token; DH / 8 lanes share a head (8 at DH = 64, 16 at 128) and a lane owns 8 consecutive dims = 4 rope pairs (32 B fp32 /
 // 16 B bf16 accesses), so a warp covers 32 / (DH / 8) heads per pass and the per-head dot product is a log2(DH / 8)-step shuffle.
-// rope_cs is [pos][DH / 2] (cos, sin).
+// rope_cs is [pos][DH / 2] (cos, sin).  Without NORM, q, k, qk_inv, the gammas and their gradients are not read and may be null.
 // xhat is rebuilt from the bf16 output as R^T q / (sqrt(DH) (gamma + 1)): where gamma_j = -1 the forward wrote y_j = 0 and xhat_j is lost, so
 // dx_j and dgamma_j come out 0 instead of -inv xhat_j (xhat . dxhat) and sum sqrt(DH) dy_j xhat_j; near -1 the bf16 error of the rope partner
 // is amplified by |gamma_partner + 1| / |gamma_j + 1|.
-template <int DH>
+template <int DH, bool NORM>
 __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_k(const float* __restrict__ dq, const float* __restrict__ dk, const __nv_bfloat16* __restrict__ q,
                                                             const __nv_bfloat16* __restrict__ k, const float* __restrict__ qk_inv, const float* __restrict__ gq,
                                                             const float* __restrict__ gk, const int* __restrict__ rope_pos, const float2* __restrict__ rope_cs,
@@ -1075,20 +1076,22 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_k(const float* __rest
   constexpr int LPH = DH / 8, HPP = 32 / LPH;
   static_assert(2 * DH <= ROW_THREADS, "one thread per gamma column in the block reduction");
   const float RS = sqrtf((float)DH);
-  __shared__ float red[WARPS_PER_BLOCK][2 * DH];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const int sub = lane % LPH, hq = lane / LPH;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);
   const int HI = H * DH;
+  // NORM only: the gamma-gradient sums, gamma + 1 and 1 / (sqrt(DH) (gamma + 1)) of the lane's 8 columns, for q and k
   float acc[2][8];
   float g1[2][8], rg[2][8];
+  if constexpr (NORM) {
 #pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    acc[0][j] = acc[1][j] = 0.f;
-    g1[0][j] = gq[sub * 8 + j] + 1.f; g1[1][j] = gk[sub * 8 + j] + 1.f;
-    rg[0][j] = fabsf(g1[0][j]) > 1e-12f ? 1.f / (RS * g1[0][j]) : 0.f;
-    rg[1][j] = fabsf(g1[1][j]) > 1e-12f ? 1.f / (RS * g1[1][j]) : 0.f;
+    for (int j = 0; j < 8; ++j) {
+      acc[0][j] = acc[1][j] = 0.f;
+      g1[0][j] = gq[sub * 8 + j] + 1.f; g1[1][j] = gk[sub * 8 + j] + 1.f;
+      rg[0][j] = fabsf(g1[0][j]) > 1e-12f ? 1.f / (RS * g1[0][j]) : 0.f;
+      rg[1][j] = fabsf(g1[1][j]) > 1e-12f ? 1.f / (RS * g1[1][j]) : 0.f;
+    }
   }
   for (int row = r0; row < r1; ++row) {
     float cs[8];   // (cos, sin) of the lane's 4 rope pairs
@@ -1099,39 +1102,53 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_k(const float* __rest
     }
     for (int h0 = 0; h0 < H; h0 += HPP) {
       const int h = h0 + hq;
-      const bool act = h < H;
+      // NORM: lanes past H join the shuffle on head 0's data and store nothing.  !NORM has no shuffle, so those lanes skip the head.
+      if constexpr (!NORM) { if (h >= H) continue; }
+      const bool act = !NORM || h < H;
       const long long off = (long long)row * HI + (act ? h : 0) * DH + sub * 8;
       // all loads of this head group (q and k, gradient and value) are issued before any arithmetic
       const float4 da[2] = {*reinterpret_cast<const float4*>(dq + off), *reinterpret_cast<const float4*>(dk + off)};
       const float4 db[2] = {*reinterpret_cast<const float4*>(dq + off + 4), *reinterpret_cast<const float4*>(dk + off + 4)};
-      const uint4 tv[2] = {*reinterpret_cast<const uint4*>(q + off), *reinterpret_cast<const uint4*>(k + off)};
-      const float invs[2] = {act ? qk_inv[(long long)row * 2 * H + h] : 0.f, act ? qk_inv[(long long)row * 2 * H + H + h] : 0.f};
+      uint4 tv[2];
+      float invs[2];
+      if constexpr (NORM) {
+        tv[0] = *reinterpret_cast<const uint4*>(q + off); tv[1] = *reinterpret_cast<const uint4*>(k + off);
+        invs[0] = act ? qk_inv[(long long)row * 2 * H + h] : 0.f; invs[1] = act ? qk_inv[(long long)row * 2 * H + H + h] : 0.f;
+      }
 #pragma unroll
       for (int which = 0; which < 2; ++which) {
         const float dr[8] = {da[which].x, da[which].y, da[which].z, da[which].w, db[which].x, db[which].y, db[which].z, db[which].w};
-        const float2 p0 = unpack2_bf16(tv[which].x), p1 = unpack2_bf16(tv[which].y), p2 = unpack2_bf16(tv[which].z), p3 = unpack2_bf16(tv[which].w);
-        const float r[8] = {p0.x, p0.y, p1.x, p1.y, p2.x, p2.y, p3.x, p3.y};
-        const float inv = invs[which];
-        float xh[8], dxh[8], dot = 0.f;
+        uint32_t w[4];
+        if constexpr (NORM) {
+          const float2 p0 = unpack2_bf16(tv[which].x), p1 = unpack2_bf16(tv[which].y), p2 = unpack2_bf16(tv[which].z), p3 = unpack2_bf16(tv[which].w);
+          const float r[8] = {p0.x, p0.y, p1.x, p1.y, p2.x, p2.y, p3.x, p3.y};
+          const float inv = invs[which];
+          float xh[8], dxh[8], dot = 0.f;
 #pragma unroll
-        for (int pr = 0; pr < 4; ++pr) {
-          const float c = cs[2 * pr], sn = cs[2 * pr + 1];
-          // un-rotate (R^T)
-          const float y0 = r[2 * pr] * c + r[2 * pr + 1] * sn, y1 = r[2 * pr + 1] * c - r[2 * pr] * sn;
-          const float dy0 = dr[2 * pr] * c + dr[2 * pr + 1] * sn, dy1 = dr[2 * pr + 1] * c - dr[2 * pr] * sn;
-          xh[2 * pr] = y0 * rg[which][2 * pr]; xh[2 * pr + 1] = y1 * rg[which][2 * pr + 1];
-          dxh[2 * pr] = dy0 * RS * g1[which][2 * pr]; dxh[2 * pr + 1] = dy1 * RS * g1[which][2 * pr + 1];
-          if (act) { acc[which][2 * pr] += dy0 * xh[2 * pr] * RS; acc[which][2 * pr + 1] += dy1 * xh[2 * pr + 1] * RS; }
-          dot += xh[2 * pr] * dxh[2 * pr] + xh[2 * pr + 1] * dxh[2 * pr + 1];
+          for (int pr = 0; pr < 4; ++pr) {
+            const float c = cs[2 * pr], sn = cs[2 * pr + 1];
+            // un-rotate (R^T)
+            const float y0 = r[2 * pr] * c + r[2 * pr + 1] * sn, y1 = r[2 * pr + 1] * c - r[2 * pr] * sn;
+            const float dy0 = dr[2 * pr] * c + dr[2 * pr + 1] * sn, dy1 = dr[2 * pr + 1] * c - dr[2 * pr] * sn;
+            xh[2 * pr] = y0 * rg[which][2 * pr]; xh[2 * pr + 1] = y1 * rg[which][2 * pr + 1];
+            dxh[2 * pr] = dy0 * RS * g1[which][2 * pr]; dxh[2 * pr + 1] = dy1 * RS * g1[which][2 * pr + 1];
+            if (act) { acc[which][2 * pr] += dy0 * xh[2 * pr] * RS; acc[which][2 * pr + 1] += dy1 * xh[2 * pr + 1] * RS; }
+            dot += xh[2 * pr] * dxh[2 * pr] + xh[2 * pr + 1] * dxh[2 * pr + 1];
+          }
+#pragma unroll
+          for (int o = 1; o < LPH; o <<= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+          if (act) {
+#pragma unroll
+            for (int pr = 0; pr < 4; ++pr) w[pr] = pack2_bf16(inv * (dxh[2 * pr] - xh[2 * pr] * dot), inv * (dxh[2 * pr + 1] - xh[2 * pr + 1] * dot));
+          }
+        } else {
+#pragma unroll
+          for (int pr = 0; pr < 4; ++pr) {
+            const float c = cs[2 * pr], sn = cs[2 * pr + 1];
+            w[pr] = pack2_bf16(dr[2 * pr] * c + dr[2 * pr + 1] * sn, dr[2 * pr + 1] * c - dr[2 * pr] * sn);     // un-rotate (R^T)
+          }
         }
-#pragma unroll
-        for (int o = 1; o < LPH; o <<= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
-        if (act) {
-          uint32_t w[4];
-#pragma unroll
-          for (int pr = 0; pr < 4; ++pr) w[pr] = pack2_bf16(inv * (dxh[2 * pr] - xh[2 * pr] * dot), inv * (dxh[2 * pr + 1] - xh[2 * pr + 1] * dot));
-          *reinterpret_cast<uint4*>(out + (long long)row * out_ld + which * HI + h * DH + sub * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
+        if (act) *reinterpret_cast<uint4*>(out + (long long)row * out_ld + which * HI + h * DH + sub * 8) = make_uint4(w[0], w[1], w[2], w[3]);
       }
     }
     // gate logits: d g = (1 - sigmoid(g)) * sum_d dO_gated * O_gated
@@ -1141,68 +1158,24 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_k(const float* __rest
       out[(long long)row * out_ld + 3 * HI + lane] = __float2bfloat16((1.f - sg) * dsum[(long long)row * H + lane]);
     }
   }
-  // gamma gradients: reduce the head groups of the warp, then the 8 warps of the block, then one atomic per column per block
+  if constexpr (NORM) {
+    // gamma gradients: reduce the head groups of the warp, then the 8 warps of the block, then one atomic per column per block
+    __shared__ float red[WARPS_PER_BLOCK][2 * DH];
 #pragma unroll
-  for (int which = 0; which < 2; ++which)
+    for (int which = 0; which < 2; ++which)
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float v = acc[which][j];
+      for (int j = 0; j < 8; ++j) {
+        float v = acc[which][j];
 #pragma unroll
-      for (int o = LPH; o < 32; o <<= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (hq == 0) red[wib][which * DH + sub * 8 + j] = v;
-    }
-  __syncthreads();
-  if (threadIdx.x < 2 * DH) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < WARPS_PER_BLOCK; ++w) t += red[w][threadIdx.x];
-    atomicAdd((threadIdx.x < DH ? dgq : dgk) + (threadIdx.x % DH), t);
-  }
-}
-
-// ------------------------------------------------------------------------------------ RoPE backward (qk_rmsnorm = False), packs d[q|k|.|gates]
-// forward (GEMM epilogue EPI_QKVG_ROPE): q = R(pos) x.  d x = R(pos)^T d q per interleaved pair; no saved values are needed.  Same lane
-// layout as qk_bwd_pack_k.
-template <int DH>
-__global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_rope_k(const float* __restrict__ dq, const float* __restrict__ dk, const int* __restrict__ rope_pos,
-                                                                 const float2* __restrict__ rope_cs, const float* __restrict__ gates, const float* __restrict__ dsum,
-                                                                 __nv_bfloat16* __restrict__ out, long long out_ld, int M, int H, int tpw) {
-  constexpr int LPH = DH / 8, HPP = 32 / LPH;
-  const int lane = threadIdx.x & 31;
-  const int sub = lane % LPH, hq = lane / LPH;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int r0 = min(M, warp * tpw), r1 = min(M, r0 + tpw);
-  const int HI = H * DH;
-  for (int row = r0; row < r1; ++row) {
-    float cs[8];   // (cos, sin) of the lane's 4 rope pairs
-    {
-      const float4* cp = reinterpret_cast<const float4*>(rope_cs + (long long)rope_pos[row] * (DH / 2) + sub * 4);
-      const float4 c0 = cp[0], c1 = cp[1];
-      cs[0] = c0.x; cs[1] = c0.y; cs[2] = c0.z; cs[3] = c0.w; cs[4] = c1.x; cs[5] = c1.y; cs[6] = c1.z; cs[7] = c1.w;
-    }
-    for (int h0 = 0; h0 < H; h0 += HPP) {
-      const int h = h0 + hq;
-      if (h >= H) continue;
-      const long long off = (long long)row * HI + h * DH + sub * 8;
-      const float4 da[2] = {*reinterpret_cast<const float4*>(dq + off), *reinterpret_cast<const float4*>(dk + off)};
-      const float4 db[2] = {*reinterpret_cast<const float4*>(dq + off + 4), *reinterpret_cast<const float4*>(dk + off + 4)};
-#pragma unroll
-      for (int which = 0; which < 2; ++which) {
-        const float dr[8] = {da[which].x, da[which].y, da[which].z, da[which].w, db[which].x, db[which].y, db[which].z, db[which].w};
-        uint32_t w[4];
-#pragma unroll
-        for (int pr = 0; pr < 4; ++pr) {
-          const float c = cs[2 * pr], sn = cs[2 * pr + 1];
-          w[pr] = pack2_bf16(dr[2 * pr] * c + dr[2 * pr + 1] * sn, dr[2 * pr + 1] * c - dr[2 * pr] * sn);     // un-rotate (R^T)
-        }
-        *reinterpret_cast<uint4*>(out + (long long)row * out_ld + which * HI + h * DH + sub * 8) = make_uint4(w[0], w[1], w[2], w[3]);
+        for (int o = LPH; o < 32; o <<= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (hq == 0) red[wib][which * DH + sub * 8 + j] = v;
       }
-    }
-    // gate logits: d g = (1 - sigmoid(g)) * sum_d dO_gated * O_gated  (as in qk_bwd_pack_k)
-    if (lane < H) {
-      const float gl = gates[(long long)row * H + lane];
-      const float sg = 1.f / (1.f + __expf(-gl));
-      out[(long long)row * out_ld + 3 * HI + lane] = __float2bfloat16((1.f - sg) * dsum[(long long)row * H + lane]);
+    __syncthreads();
+    if (threadIdx.x < 2 * DH) {
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < WARPS_PER_BLOCK; ++w) t += red[w][threadIdx.x];
+      atomicAdd((threadIdx.x < DH ? dgq : dgk) + (threadIdx.x % DH), t);
     }
   }
 }
@@ -1223,6 +1196,21 @@ int num_sms();
 
 using namespace tfx;
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
+
+// tfx_qk_bwd_pack(_rope)(_d128); `name` is the entry point's name for error messages.  Without NORM the norm pointers are null.
+template <int DH, bool NORM>
+static int qk_bwd_pack(const char* name, const float* dq, const float* dk, const void* q_bf16, const void* k_bf16, const float* qk_inv, const float* q_gamma,
+                       const float* k_gamma, const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum, void* dqkvg_bf16, long long out_ld,
+                       float* dq_gamma, float* dk_gamma, int M, int H, void* stream) {
+  if (M <= 0) return 0;
+  constexpr int max_heads = 2048 / DH;     // inner width up to 2048; at 64 also one gate column per lane
+  TFX_REQUIRE(H >= 1 && H <= max_heads, "%s: heads %d out of range [1, %d]", name, H, max_heads);
+  const int tpw = 8;
+  qk_bwd_pack_k<DH, NORM><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, (const __nv_bfloat16*)q_bf16, (const __nv_bfloat16*)k_bf16, qk_inv, q_gamma,
+                                                                            k_gamma, rope_pos, (const float2*)rope_cs, gates, dsum, (__nv_bfloat16*)dqkvg_bf16, out_ld,
+                                                                            dq_gamma, dk_gamma, M, H, tpw);
+  return check_launch(name);
+}
 
 extern "C" {
 
@@ -1404,43 +1392,27 @@ int tfx_clean_flow_bwd(float* dmod_inout, float* dmodtok_neg, const int* row_tok
 int tfx_qk_bwd_pack(const float* dq, const float* dk, const void* q_bf16, const void* k_bf16, const float* qk_inv, const float* q_gamma, const float* k_gamma,
                     const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum, void* dqkvg_bf16, long long out_ld,
                     float* dq_gamma, float* dk_gamma, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(H >= 1 && H <= 32, "qk_bwd_pack: heads %d out of range", H);
-  const int tpw = 8;
-  qk_bwd_pack_k<64><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, (const __nv_bfloat16*)q_bf16, (const __nv_bfloat16*)k_bf16, qk_inv, q_gamma, k_gamma, rope_pos,
-                                                                     (const float2*)rope_cs, gates, dsum, (__nv_bfloat16*)dqkvg_bf16, out_ld, dq_gamma, dk_gamma, M, H, tpw);
-  return check_launch("qk_bwd_pack");
+  return qk_bwd_pack<64, true>("qk_bwd_pack", dq, dk, q_bf16, k_bf16, qk_inv, q_gamma, k_gamma, rope_pos, rope_cs, gates, dsum, dqkvg_bf16, out_ld,
+                               dq_gamma, dk_gamma, M, H, stream);
 }
 
 int tfx_qk_bwd_pack_rope(const float* dq, const float* dk, const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16,
                          long long out_ld, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(H >= 1 && H <= 32, "qk_bwd_pack_rope: heads %d out of range", H);
-  const int tpw = 8;
-  qk_bwd_pack_rope_k<64><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, rope_pos, (const float2*)rope_cs, gates, dsum_mh, (__nv_bfloat16*)dqkvg_bf16, out_ld, M, H, tpw);
-  return check_launch("qk_bwd_pack_rope");
+  return qk_bwd_pack<64, false>("qk_bwd_pack_rope", dq, dk, nullptr, nullptr, nullptr, nullptr, nullptr, rope_pos, rope_cs, gates, dsum_mh, dqkvg_bf16, out_ld,
+                                nullptr, nullptr, M, H, stream);
 }
 
 int tfx_qk_bwd_pack_d128(const float* dq, const float* dk, const void* q_bf16, const void* k_bf16, const float* qk_inv, const float* q_gamma, const float* k_gamma,
                          const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum, void* dqkvg_bf16, long long out_ld,
                          float* dq_gamma, float* dk_gamma, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(H >= 1 && H <= 16, "qk_bwd_pack_d128: heads %d out of range [1, 16]", H);
-  const int tpw = 8;
-  qk_bwd_pack_k<128><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, (const __nv_bfloat16*)q_bf16, (const __nv_bfloat16*)k_bf16, qk_inv, q_gamma, k_gamma,
-                                                                           rope_pos, (const float2*)rope_cs, gates, dsum, (__nv_bfloat16*)dqkvg_bf16, out_ld, dq_gamma,
-                                                                           dk_gamma, M, H, tpw);
-  return check_launch("qk_bwd_pack_d128");
+  return qk_bwd_pack<128, true>("qk_bwd_pack_d128", dq, dk, q_bf16, k_bf16, qk_inv, q_gamma, k_gamma, rope_pos, rope_cs, gates, dsum, dqkvg_bf16, out_ld,
+                                dq_gamma, dk_gamma, M, H, stream);
 }
 
 int tfx_qk_bwd_pack_rope_d128(const float* dq, const float* dk, const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16,
                               long long out_ld, int M, int H, void* stream) {
-  if (M <= 0) return 0;
-  TFX_REQUIRE(H >= 1 && H <= 16, "qk_bwd_pack_rope_d128: heads %d out of range [1, 16]", H);
-  const int tpw = 8;
-  qk_bwd_pack_rope_k<128><<<chunk_grid(M, tpw), ROW_THREADS, 0, ST(stream)>>>(dq, dk, rope_pos, (const float2*)rope_cs, gates, dsum_mh, (__nv_bfloat16*)dqkvg_bf16,
-                                                                                out_ld, M, H, tpw);
-  return check_launch("qk_bwd_pack_rope_d128");
+  return qk_bwd_pack<128, false>("qk_bwd_pack_rope_d128", dq, dk, nullptr, nullptr, nullptr, nullptr, nullptr, rope_pos, rope_cs, gates, dsum_mh, dqkvg_bf16,
+                                 out_ld, nullptr, nullptr, M, H, stream);
 }
 
 }  // extern "C"
