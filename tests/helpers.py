@@ -12,6 +12,25 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 BF16, F32 = torch.bfloat16, torch.float32
 SENT = -77.5                          # exact in bf16 and fp32
 
+# fp32 accumulation of the wgmma main loop, relative to |A| |B|^T: 1.6e-6 is the bound measured over K <= 2752 = 43 k-blocks of 64
+# (5.4e-7 there, test_block_epilogues_gpu.py).  Rounding errors of random-sign sums grow like the square root of their length, so the bound
+# grows with sqrt(kb / 43) above that.  Measured on an H100 80GB HBM3 (700 W power limit), worst over the files that use it: 7.0e-7 at 64
+# k-blocks (gemm_resid, K = 4096; 0.36 of c_acc(64)), 7.4e-7 at 86 (gemm_resid, K = 5504; 0.33), 6.8e-7 at 128 and 8.3e-7 at 172 (the gemm_store
+# replay, where the dgrad du = dvg W1 of the d1536 and d2048 models runs them; 0.25 and 0.26), 1.4e-6 at 384 (the d2048 conditioning dgrad; 0.29).
+C_ACC0, KB0 = 1.6e-6, 43
+
+
+def c_acc(kb):
+    """the accumulator bound of a GEMM work item that runs kb k-blocks of 64"""
+    return C_ACC0 * max(1., (kb / KB0) ** 0.5)
+
+
+def show_c_acc(shown, kb, measured):
+    """keep a measured accumulator error (relative to |A| |B|^T) as the file's worst, and past KB0 k-blocks also per k-block count"""
+    keys = ['c_acc (measured)'] + ([f'c_acc (measured) at kb = {kb}'] if kb > KB0 else [])
+    for k in keys:
+        shown[k] = max(shown.get(k, 0.), measured)
+
 
 # ------------------------------------------------------------------------------------------------ float64 kernel tests
 class Checks:
@@ -21,7 +40,8 @@ class Checks:
     def __init__(self, what, shown):
         self.what, self.shown, self.bad = what, shown, []
 
-    def __call__(self, name, got, ref, bound):
+    def __call__(self, name, got, ref, bound, row0 = 0):
+        """row0: the first row of got / ref / bound when they are a row chunk of the output (for the failure report)"""
         got = got.double()
         err = (got - ref).abs()
         ratio = (err / bound.clamp_min(1e-300)).nan_to_num(nan = float('inf'))
@@ -32,7 +52,8 @@ class Checks:
             self.bad.append(f'{name}: non-finite values')
         elif r > 1:
             i = np.unravel_index(int(ratio.argmax()), tuple(ratio.shape))
-            self.bad.append(f'{name}: {int((ratio > 1).sum())} values off, worst err / bound {r:.3e} at {tuple(int(x) for x in i)} '
+            at = (int(i[0]) + row0,) + tuple(int(x) for x in i[1:])
+            self.bad.append(f'{name}: {int((ratio > 1).sum())} values off, worst err / bound {r:.3e} at {at} '
                             f'(got {got[i].item():.6e}, ref {ref[i].item():.6e})')
 
     def true(self, name, ok):

@@ -347,6 +347,11 @@ def test_cast_pack_multi_paths(ops):
 ENGINE_MODELS = {
     'd512': dict(num_text_tokens = 256, dim_latent = 384, modality_default_shape = (256,), transformer = dict(dim = 512, depth = 2)),
     'd128': dict(num_text_tokens = 64, dim_latent = 32, modality_default_shape = (4,), transformer = dict(dim = 128, depth = 2, heads = 2)),
+    'd1536': dict(num_text_tokens = 64, dim_latent = (32, 16), modality_default_shape = ((4,), (2,)), transformer = dict(dim = 1536, depth = 2, heads = 8)),
+    'd2048': dict(num_text_tokens = 64, dim_latent = (32, 16), modality_default_shape = ((4,), (2,)),
+                  transformer = dict(dim = 2048, depth = 2, heads = 16, dim_head = 128)),
+    'd384h3x128vres': dict(num_text_tokens = 64, dim_latent = 32, modality_default_shape = (4,),
+                           transformer = dict(dim = 384, depth = 3, heads = 3, dim_head = 128, use_value_residual = True)),
 }
 
 
@@ -363,7 +368,10 @@ def packed_layout(eng):
         wq = torch.zeros(eng.NQ, D, device = 'cuda')
         wq[:2 * HI] = P(f'{pre}.1.fn.to_qk.0.weight'); wq[2 * HI:3 * HI] = P(f'{pre}.1.fn.to_v.0.weight'); wq[3 * HI:3 * HI + H] = P(f'{pre}.1.fn.to_gates.0.weight')
         if f'{pre}.1.fn.to_learned_value_residual.0.weight' in eng.named:
-            wq[3 * HI + H:3 * HI + 2 * H] = P(f'{pre}.1.fn.to_learned_value_residual.0.weight')
+            # the mix rows start at the first even row behind the gates, so that the bf16 pairs of their gradient columns stay 4-byte
+            # aligned: one pad row between them at an odd head count (dim_head 128 only)
+            mix = 3 * HI + H + H % 2
+            wq[mix:mix + H] = P(f'{pre}.1.fn.to_learned_value_residual.0.weight')
         out[f'qkvg{i}'] = wq
         out[f'wo{i}'] = P(f'{pre}.1.fn.to_out.1.weight')
         w1 = torch.zeros(2 * Ip, D, device = 'cuda'); w1[ok] = P(f'{pre}.2.fn.net.0.weight')[src[ok]]

@@ -9,7 +9,8 @@ Each kernel is called through the C ABI with the argument patterns of engine.for
 
 Reference and bounds (every check is |got - ref| <= bound element-wise; the worst err / bound of each check is printed, run with -s):
   - GEMM part: y64 = u.double() @ W.double().T from the same bf16 operands, mag = |u| @ |W|^T in float64.  The fp32 tensor-core
-    accumulation is bounded by C_ACC * mag per element.
+    accumulation over kb = ceil(K / 64) k-blocks is bounded by c_acc(kb) * mag per element (helpers.py: 1.6e-6 up to 43 k-blocks, growing
+    with sqrt(kb / 43) past that); C_ACC below stands for c_acc(kb) of the GEMM at hand.
   - epilogue outputs are computed in float64 from y64.  A bf16 output may differ by 2^-8 |ref| (the rounding of the cast) plus the
     accumulator bound carried through the epilogue; for q / k that is 8 |gamma + 1| inv times the rope pair's C_ACC * mag, plus the
     error of inv, plus a few fp32 roundings (2^-24 relative each).  fp32 outputs (gates, mix, qk_inv, x_out) get the accumulator term
@@ -31,7 +32,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import SENT, Checks as _Checks, cluster_mode, gen, guarded, same_bits, untouched  # noqa: F401  (cluster_mode: a fixture)
+from helpers import SENT, Checks as _Checks, c_acc, cluster_mode, gen, guarded, same_bits, show_c_acc, untouched  # noqa: F401  (cluster_mode: a fixture)
 from transfusion_pytorch_b200 import _lib, engine as E
 from oracle.dropout_mask import keep_mask, scale as drop_scale, SITE_FFN
 
@@ -41,8 +42,12 @@ U8, U24 = 2.0 ** -8, 2.0 ** -24       # bf16 cast, one fp32 rounding (relative)
 M_ROWS = 9011
 N_POS = 16384                         # RoPE table length; positions run to its last entry
 ZERO_ROW = 4321                       # an all-zero row of u in the QKVG test
+# float64 values of [rows, 2 Ip] per row chunk of the GEGLU forward reference: one chunk up to D = 1024 (M_ROWS x 5504), two at 1536 and
+# 2048, where the whole reference would peak past 10 GB of device memory (measured on the H100: 10.3 GiB at D = 2048 in one chunk, 5.8 GiB in
+# two)
+REF_VALUES = 50_000_000
 
-C_ACC = 1.6e-6     # fp32 accumulation of the wgmma GEMMs, relative to |u| @ |W|^T; measured 5.4e-7 (x_out, K <= 2752; QKVG gates 4.0e-7)
+# fp32 accumulation of the wgmma GEMMs: c_acc(kb) of helpers.py, relative to |u| @ |W|^T; measured 5.4e-7 (x_out, K <= 2752; QKVG gates 4.0e-7)
 REL_SUM = 1e-6     # column sums / atomics, relative to the sum of |terms|; measured 1.2e-7 (resid_bwd dzgate)
 PHI_ABS = 7.5e-8   # Abramowitz-Stegun 7.1.26 in gelu_parts: |erf error| <= 1.5e-7, so Phi is off by at most half of it (not a fit)
 # Measured worst err / bound of the checks (same H100 run, with the constants above): every bf16 output 0.99 - 0.996 (the cast's rounding,
@@ -78,6 +83,11 @@ def Checks(what):
 def gemm64(a, w):
     a64, w64 = a.double(), w.double()
     return a64 @ w64.t(), a64.abs() @ w64.abs().t()
+
+
+def kblocks(a):
+    """k-blocks of 64 of a GEMM over the columns of its operand a"""
+    return (a.shape[1] + 63) // 64
 
 
 def cond_runs(M, nc, seed):
@@ -150,16 +160,18 @@ def run_qkvg(ops, x, tt, M = M_ROWS, rows = None, kv = None):
     return out
 
 
-def qk_forward_ref(x, mag, gamma, c, s):
-    """float64 q (or k) of one GEMM section x [M, H, dh] and its bound; also returns inv64 and the bound on inv's relative error"""
+def qk_forward_ref(x, mag, gamma, c, s, kb):
+    """float64 q (or k) of one GEMM section x [M, H, dh] over kb k-blocks and its bound; also returns inv64 and the bound on inv's relative
+    error"""
+    ca = c_acc(kb)
     nrm = x.norm(dim = -1, keepdim = True)
     inv = 1. / nrm.clamp_min(1e-12)
     g1 = gamma.double() + 1.
     rt = x.shape[-1] ** 0.5                               # sqrt(dh): 8 at dh = 64
     y = x * inv * rt * g1
     ref = rope64(y, c, s)
-    rel_inv = C_ACC * (x.abs() * mag).sum(-1, keepdim = True) / (nrm * nrm).clamp_min(1e-300) + 40 * U24
-    Ey = rt * g1.abs() * inv * (C_ACC * mag + x.abs() * rel_inv) + 3 * U24 * y.abs()
+    rel_inv = ca * (x.abs() * mag).sum(-1, keepdim = True) / (nrm * nrm).clamp_min(1e-300) + 40 * U24
+    Ey = rt * g1.abs() * inv * (ca * mag + x.abs() * rel_inv) + 3 * U24 * y.abs()
     Ep = pair_sum(Ey + 3 * U24 * y.abs())
     return ref, U8 * ref.abs() + (1 + U8) * Ep, inv, rel_inv
 
@@ -174,26 +186,28 @@ def test_gemm_qkvg_vs_float64(ops, cluster_mode, D, H, mix, dh = 64):
     tag = '' if dh == 64 else f' dh={dh}'
     ck = Checks(f'qkvg{tag} D={D} H={H}')
     y, mag = gemm64(x['u'], x['W'])
+    kb = kblocks(x['u'])
+    ca = c_acc(kb)
     cs = t[x['pos'].long()].double()
     c, s = cs[:, None, :, 0], cs[:, None, :, 1]
     for which, gam in ((0, x['gq']), (1, x['gk'])):
         sec = slice(which * HI, (which + 1) * HI)
-        ref, bound, inv, rel_inv = qk_forward_ref(y[:, sec].reshape(M, H, dh), mag[:, sec].reshape(M, H, dh), gam, c, s)
+        ref, bound, inv, rel_inv = qk_forward_ref(y[:, sec].reshape(M, H, dh), mag[:, sec].reshape(M, H, dh), gam, c, s, kb)
         name = 'qk'[which]
         ck(f'qkvg{tag} {name}', o[name].reshape(M, H, dh), ref, bound)
         ck(f'qkvg{tag} inv_{name}', o['inv'][:, which * H:(which + 1) * H], inv[..., 0], inv[..., 0] * rel_inv[..., 0] * (1 + U8))
-    ck(f'qkvg{tag} v', o['v'], y[:, 2 * HI:3 * HI], U8 * y[:, 2 * HI:3 * HI].abs() + (1 + U8) * C_ACC * mag[:, 2 * HI:3 * HI])
+    ck(f'qkvg{tag} v', o['v'], y[:, 2 * HI:3 * HI], U8 * y[:, 2 * HI:3 * HI].abs() + (1 + U8) * ca * mag[:, 2 * HI:3 * HI])
     m0 = 3 * HI + (H + 1) // 2 * 2                       # the mix rows start at an even row (an odd H exists at dh = 128 only)
     gsl, msl = slice(3 * HI, 3 * HI + H), slice(m0, m0 + H)
-    ck(f'qkvg{tag} gates', o['gates'], y[:, gsl], C_ACC * mag[:, gsl])
-    c_acc = ((o['gates'].double() - y[:, gsl]).abs() / mag[:, gsl].clamp_min(1e-300)).max().item()
+    ck(f'qkvg{tag} gates', o['gates'], y[:, gsl], ca * mag[:, gsl])
+    acc = ((o['gates'].double() - y[:, gsl]).abs() / mag[:, gsl].clamp_min(1e-300)).max().item()
     if mix:
-        ck(f'qkvg{tag} mix', o['mix'], y[:, msl], C_ACC * mag[:, msl])
-        c_acc = max(c_acc, ((o['mix'].double() - y[:, msl]).abs() / mag[:, msl].clamp_min(1e-300)).max().item())
+        ck(f'qkvg{tag} mix', o['mix'], y[:, msl], ca * mag[:, msl])
+        acc = max(acc, ((o['mix'].double() - y[:, msl]).abs() / mag[:, msl].clamp_min(1e-300)).max().item())
     else:
         ck.true('mix buffer untouched without mix_pre', untouched(o['mix_buf']))
-    SHOWN['c_acc (measured)'] = max(SHOWN.get('c_acc (measured)', 0.), c_acc)
-    print(f'qkvg D={D} H={H}: measured accumulator error {c_acc:.3g} of |u| |W|^T')
+    show_c_acc(SHOWN, kb, acc)
+    print(f'qkvg D={D} H={H}: measured accumulator error {acc:.3g} of |u| |W|^T')
     # the all-zero row: q and k exactly 0, inv = 1 / 1e-12 (the clamp), nothing non-finite
     z = ZERO_ROW
     ck.true('zero row: q, k exactly 0', bool((o['q'][z] == 0).all() and (o['k'][z] == 0).all()))
@@ -322,9 +336,9 @@ def test_qk_bwd_pack_at_gamma_minus_one(ops, dh = 64):
 
 
 # ================================================================================================ gemm_resid
-def resid_bounds(y, mag, x_res, sc):
-    """y64 (+ bias), the bound of bf16(y), x_out = x_res + y sc and its fp32 bound (sc None: plain residual add)"""
-    Ey = C_ACC * mag + U24 * y.abs()
+def resid_bounds(y, mag, kb, x_res, sc):
+    """y64 (+ bias) over kb k-blocks, the bound of bf16(y), x_out = x_res + y sc and its fp32 bound (sc None: plain residual add)"""
+    Ey = c_acc(kb) * mag + U24 * y.abs()
     ys = y if sc is None else y * sc
     xo = x_res + ys
     Exo = (1. if sc is None else sc.abs()) * Ey + 3 * U24 * (x_res.abs() + 2 * ys.abs())
@@ -346,16 +360,16 @@ def test_gemm_resid_vs_float64(ops, cluster_mode, D, H, mix):
     ck = Checks(f'resid D={D} H={H}')
     xo_buf, xo = guarded(M, D, F32); yb_buf, yb = guarded(M, D, BF16); xb_buf, xb = guarded(M, D, BF16)
 
-    def check_out(tag, y, mag, s, y_out, x32, x16):
-        by, ref, Exo = resid_bounds(y, mag, x_res.double(), s)
+    def check_out(tag, y, mag, kb, s, y_out, x32, x16):
+        by, ref, Exo = resid_bounds(y, mag, kb, x_res.double(), s)
         if y_out is not None:
             ck(f'resid {tag} y', y_out, y, by)
         if x32 is not None:
             ck(f'resid {tag} x_out', x32, ref, Exo)
-            # accumulator error implied by x_out once its fp32 roundings are taken off: the long-K GEMMs of the layer (K up to 2752)
+            # accumulator error implied by x_out once its fp32 roundings are taken off: the long-K GEMMs of the layer (K up to 5504)
             smag = (1. if s is None else s.abs()) * mag
-            c_acc = (((x32.double() - ref).abs() - (Exo - C_ACC * smag)).clamp_min(0) / smag.clamp_min(1e-300)).max().item()
-            SHOWN['c_acc (measured)'] = max(SHOWN.get('c_acc (measured)', 0.), c_acc)
+            acc = (((x32.double() - ref).abs() - (Exo - c_acc(kb) * smag)).clamp_min(0) / smag.clamp_min(1e-300)).max().item()
+            show_c_acc(SHOWN, kb, acc)
         if x16 is not None:
             ck(f'resid {tag} x_out_bf16', x16, ref, U8 * ref.abs() + (1 + U8) * Exo)
 
@@ -364,11 +378,11 @@ def test_gemm_resid_vs_float64(ops, cluster_mode, D, H, mix):
     Wo = (torch.randn(D, HI, device = 'cuda', generator = g) / HI ** 0.5).to(BF16)
     ops.gemm_resid(att, HI, None, 0, 0, Wo, HI, M, D, HI, None, x_res, xo, None, yb, cond, zg[:, w * D:], Wn * D, ls)
     y, mag = gemm64(att, Wo)
-    check_out('attn', y, mag, sc, yb, xo, None)
+    check_out('attn', y, mag, kblocks(att), sc, yb, xo, None)
     ck.true('attn: guard rows untouched', untouched(xo_buf[M]) and untouched(yb_buf[M]) and untouched(xb_buf))
     # text-only model: no condition table, layerscale on every row
     ops.gemm_resid(att, HI, None, 0, 0, Wo, HI, M, D, HI, None, x_res, xo, None, None, None, None, 0, ls)
-    check_out('text-only', y, mag, (ls.double() + 1.).expand(M, D), None, xo, None)
+    check_out('text-only', y, mag, kblocks(att), (ls.double() + 1.).expand(M, D), None, xo, None)
     # FFN out-projection: K = Ip (pad columns of h and W2 are 0), bias; once with fp32 x_out, once with the bf16 copy only
     h = torch.randn(M, Ip, device = 'cuda', generator = g).to(BF16); h[:, inner:] = 0
     W2 = (torch.randn(D, Ip, device = 'cuda', generator = g) / inner ** 0.5).to(BF16); W2[:, inner:] = 0
@@ -376,10 +390,10 @@ def test_gemm_resid_vs_float64(ops, cluster_mode, D, H, mix):
     y, mag = gemm64(h, W2)
     y = y + b2.double()
     ops.gemm_resid(h, Ip, None, 0, 0, W2, Ip, M, D, Ip, b2, x_res, xo, None, yb, cond, zg[:, w * D:], Wn * D, ls)
-    check_out('ffn', y, mag, sc, yb, xo, None)
+    check_out('ffn', y, mag, kblocks(h), sc, yb, xo, None)
     yb.fill_(SENT)
     ops.gemm_resid(h, Ip, None, 0, 0, W2, Ip, M, D, Ip, b2, x_res, None, xb, yb, cond, zg[:, w * D:], Wn * D, ls)
-    check_out('ffn bf16-only', y, mag, sc, yb, None, xb)
+    check_out('ffn bf16-only', y, mag, kblocks(h), sc, yb, None, xb)
     ck.true('ffn: guard rows untouched', untouched(xo_buf[M]) and untouched(yb_buf[M]) and untouched(xb_buf[M]))
     # U-Net skip projection: x_a = x_in + [x_in | skip] W_skip^T, the concatenation read as two operands (K1 = D)
     xin_b = torch.randn(M, D, device = 'cuda', generator = g).to(BF16); skip_b = torch.randn(M, D, device = 'cuda', generator = g).to(BF16)
@@ -387,7 +401,7 @@ def test_gemm_resid_vs_float64(ops, cluster_mode, D, H, mix):
     xo.fill_(SENT)
     ops.gemm_resid(xin_b, D, skip_b, D, D, Wsk, 2 * D, M, D, 2 * D, None, x_res, xo, None, None, None, None, 0, None)
     y, mag = gemm64(torch.cat((xin_b, skip_b), 1), Wsk)
-    check_out('skip', y, mag, None, None, xo, None)
+    check_out('skip', y, mag, kblocks(Wsk), None, None, xo, None)
     ck.true('skip: guard row untouched', untouched(xo_buf[M]))
     ck.done()
 
@@ -502,27 +516,39 @@ def test_gemm_geglu_vs_float64(ops, cluster_mode, D, H, mix):
     Wp, bp, src = packed_w1(D, inner, g)
     u = torch.randn(M, D, device = 'cuda', generator = g).to(BF16)
     ck = Checks(f'geglu D={D} inner={inner}')
-    y, mag = gemm64(u, Wp)
-    y = y + bp.double()
-    Ey = C_ACC * mag + U24 * y.abs()
-    v, gt = split_vg(y, Ip)
-    Ev, Eg = split_vg(Ey, Ip)
-    Phi, phi = phi_cdf(gt)
-    dPhi, _ = gelu_err(gt)
-    href = v * gt * Phi
-    Eh = v.abs() * (Phi + gt.abs() * phi) * Eg + (gt * Phi).abs() * Ev + v.abs() * gt.abs() * dPhi + 4 * U24 * href.abs()
     keep = ffn_keep(DROP_KEY, DROP_P, DROP_LAYER, M, Ip)
     sc = drop_scale(DROP_P)
+    out = {}
     for drop in (False, True):
         vg_buf, vg = guarded(M, 2 * Ip, BF16); h_buf, h = guarded(M, Ip, BF16)
         if drop:
             ops.gemm_geglu_drop(u, D, Wp, D, bp, M, 2 * Ip, D, vg, h, dev_key(DROP_KEY), DROP_P, DROP_LAYER)
         else:
             ops.gemm_geglu(u, D, Wp, D, bp, M, 2 * Ip, D, vg, h)
+        out[drop] = vg_buf, vg, h_buf, h
+    # the float64 reference in row chunks of at most REF_VALUES entries of [rows, 2 Ip]
+    n_chunks = -(-M * 2 * Ip // REF_VALUES)
+    step = -(-M // n_chunks)
+    for r0 in range(0, M, step):
+        rs = slice(r0, min(r0 + step, M))
+        y, mag = gemm64(u[rs], Wp)
+        y = y + bp.double()
+        Ey = c_acc(kblocks(u)) * mag + U24 * y.abs()
+        v, gt = split_vg(y, Ip)
+        Ev, Eg = split_vg(Ey, Ip)
+        Phi, phi = phi_cdf(gt)
+        dPhi, _ = gelu_err(gt)
+        href = v * gt * Phi
+        Eh = v.abs() * (Phi + gt.abs() * phi) * Eg + (gt * Phi).abs() * Ev + v.abs() * gt.abs() * dPhi + 4 * U24 * href.abs()
+        for drop in (False, True):
+            _, vg, _, h = out[drop]
+            tag = 'geglu_drop' if drop else 'geglu'
+            ck(f'{tag} vg', vg[rs], y, U8 * y.abs() + (1 + U8) * Ey, row0 = r0)
+            want, Ew = (href * keep[rs] * sc, (Eh + U24 * href.abs()) * sc) if drop else (href, Eh)
+            ck(f'{tag} h', h[rs, :inner], want[:, :inner], U8 * want[:, :inner].abs() + (1 + U8) * Ew[:, :inner], row0 = r0)
+    for drop in (False, True):
+        vg_buf, vg, h_buf, h = out[drop]
         tag = 'geglu_drop' if drop else 'geglu'
-        ck(f'{tag} vg', vg, y, U8 * y.abs() + (1 + U8) * Ey)
-        want, Ew = (href * keep * sc, (Eh + U24 * href.abs()) * sc) if drop else (href, Eh)
-        ck(f'{tag} h', h[:, :inner], want[:, :inner], U8 * want[:, :inner].abs() + (1 + U8) * Ew[:, :inner])
         ck.true(f'{tag}: pad columns of h exactly 0', bool((h[:, inner:].view(torch.int16) == 0).all()))
         if drop:
             ck.true('dropped h entries exactly 0', bool((h[:, :inner][~keep[:, :inner]].view(torch.int16) == 0).all()))

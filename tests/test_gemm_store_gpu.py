@@ -4,12 +4,15 @@
     out_bf16    = bf16(alpha A B^T + bias)
 
 Two tests:
-  - the replay: every distinct gemm_store call of one eager forward + backward of four models (d128 with two modality types and one
-    condition row, a d512 config-2-like model over 4096 tokens, a text-only d128 model, a Self-Flow model), recorded on the engine's Ops
-    instance and replayed with fresh operands of the same geometry, pitches, output alignment (address mod 16), row offsets, alpha,
-    accumulate and split-K.  The test asserts that the recorded set still holds the edge cases below, so it cannot lose them silently when
-    the engine changes: K < 64, N < 32, M <= 2, K <= 2 with both operands MN-major, odd N through row_off, a row offset that is not a
-    multiple of 4, k_splits > 1, a bf16-only output.
+  - the replay: every distinct gemm_store call of one eager forward + backward of seven models (d128 with two modality types and one
+    condition row, a d512 config-2-like model over 4096 tokens, a text-only d128 model, a Self-Flow model, the d1536 (8 heads of 64) and
+    d2048 (16 heads of 128) models of the wide training-step fixtures, a d384 model with 3 heads of 128 and the learned value residual),
+    recorded on the engine's Ops instance and replayed with fresh operands of the same geometry, pitches, output alignment (address mod 16),
+    row offsets, alpha, accumulate and split-K.  The test asserts that the recorded set still holds the edge cases below, so it cannot lose
+    them silently when the engine changes: K < 64, N < 32, M <= 2, K <= 2 with both operands MN-major, odd N through row_off, a row offset
+    that is not a multiple of 4, k_splits > 1, a bf16-only output, a dgrad (A K-major, B MN-major, no split) over more than 128 k-blocks
+    (du = dvg W1 at d2048: 172), a wgrad with more than 8192 output rows through row_off with -1 rows (W1 at d2048: 11008 rows, 86 of them
+    pad), and one -1 row between mapped rows (the QKVG wgrad at an odd head count, whose value-residual mix rows start at an even row).
   - explicit edges the ABI allows, under every schedule a launch can take (ping-pong single CTA, ping-pong 2-CTA clusters, the 256 x 128
     wide tile): K in {1, 8, 63, 64, 65, 390}, M in {1, 2, 127, 129, 257, 300, 40000} (40000: several tiles per CTA, an odd tile count),
     N in {1, 31, 33, 390, 1365}, all four operand majors; each case stores fp32 + bf16 with alpha and bias (bf16 pitch not a multiple of
@@ -28,26 +31,26 @@ Reference and bound (|got - ref| <= bound element-wise, worst err / bound printe
 import pytest
 import torch
 
-from helpers import SENT, Checks as _Checks, gen, load_golden, same_bits
+from helpers import SENT, Checks as _Checks, c_acc, gen, load_golden, show_c_acc
 from test_selfflow_cpu import selfflow_noise, selfflow_wrapper
 from transfusion_pytorch_b200 import Transfusion, _lib, synth
 
 pytestmark = pytest.mark.gpu
 BF16, F32 = torch.bfloat16, torch.float32
 U8, U24 = 2.0 ** -8, 2.0 ** -24
-# fp32 accumulation of the wgmma main loop, relative to |A| |B|^T: 1.6e-6 is the bound test_block_epilogues_gpu.py holds (measured
-# 5.4e-7 there, K up to 2752 = 43 k-blocks).  Rounding errors of random-sign sums grow like the square root of their length, so the
-# bound grows with sqrt(kb / 43) above that.  Measured here on an H100 80GB HBM3 (700 W power limit): at most 4.3e-7 of |A| |B|^T (kb = 96,
-# K = 6144), 0.20 of C_ACC(kb) over every call of the file.
-C_ACC0, KB0 = 1.6e-6, 43
+# fp32 accumulation of the wgmma main loop: c_acc(kb) of helpers.py, C_ACC0 = 1.6e-6 of |A| |B|^T up to 43 k-blocks, growing with
+# sqrt(kb / 43) above that.  Measured here on an H100 80GB HBM3 (700 W power limit): at most 1.4e-6 of |A| |B|^T (kb = 384, K = 24576: the
+# conditioning dgrad of the d2048 model), 0.29 of C_ACC(kb) over every call of the file.
 # Measured worst err / bound (same run): bf16 outputs 0.98 - 0.996 (the cast's rounding, which the bound states exactly); fp32 outputs of
-# the replay <= 0.33 (the K = 1 wgrads through row_off), of the explicit edges <= 0.43.
+# the replay <= 0.33 (the K = 1 wgrads through row_off), of the explicit edges <= 0.43.  Recording the seven models takes 15 s, the replay
+# 1.3 s.
+# The float64 reference and checks of one call run over row chunks of at most REF_VALUES outputs (a dozen [rows, N] float64 / int64 arrays
+# each): every explicit edge and every call of the d512 and smaller models is one chunk; the largest product, the d2048 model's
+# conditioning-table wgrad (24576 x 8192 outputs), takes 12.  Measured on the same H100: whole, its checks peaked at 20.3 GiB of device
+# memory; in chunks the replay's checks peak at 4.6 GiB, over the 5.8 GiB that recording the seven models leaves allocated.
+REF_VALUES = 1 << 24
 
 SHOWN = {}
-
-
-def c_acc(kb):
-    return C_ACC0 * max(1., (kb / KB0) ** 0.5)
 
 
 @pytest.fixture(scope = 'module')
@@ -90,36 +93,44 @@ class Out:
     def __init__(self, M, N, ld, dtype, align, row_off, init, g):
         esz = torch.finfo(dtype).bits // 8
         assert align % esz == 0
-        pre = align // esz
-        offs = row_off.long() if row_off is not None else torch.arange(M, device = 'cuda') * ld
-        self.valid = offs >= 0
-        end = int(offs[self.valid].max()) + N if bool(self.valid.any()) else 0
+        self.pre, self.N = align // esz, N
+        self.offs = row_off.long() if row_off is not None else torch.arange(M, device = 'cuda') * ld
+        self.valid = self.offs >= 0
+        end = int(self.offs[self.valid].max()) + N if bool(self.valid.any()) else 0
         if row_off is None:
             end = max(end, (M + 1) * ld)
-        size = pre + end + 37
+        size = self.pre + end + 37
         if init == 'sentinel':
             self.flat = torch.full((size,), SENT, dtype = dtype, device = 'cuda')
         else:
             self.flat = torch.randn(size, device = 'cuda', generator = g).to(dtype)
         assert self.flat.data_ptr() % 16 == 0
         self.flat0 = self.flat.clone()
-        self.ptr = self.flat[pre:]
-        self.idx = pre + offs[self.valid][:, None] + torch.arange(N, device = 'cuda')[None]
+        self.ptr = self.flat[self.pre:]
+        self.written = torch.zeros_like(self.flat, dtype = torch.bool)
 
-    def got(self):
-        return self.flat[self.idx]
+    def idx(self, rows):
+        """flat indices of the stored rows among `rows` (a slice of the M output rows)"""
+        offs = self.offs[rows]
+        return self.pre + offs[offs >= 0][:, None] + torch.arange(self.N, device = 'cuda')[None]
 
-    def initial(self):
-        return self.flat0[self.idx].double()
+    def got(self, rows):
+        i = self.idx(rows)
+        self.written[i.reshape(-1)] = True
+        return self.flat[i]
+
+    def initial(self, rows):
+        return self.flat0[self.idx(rows)].double()
 
     def rest_untouched(self):
-        keep = torch.ones_like(self.flat, dtype = torch.bool)
-        keep[self.idx.reshape(-1)] = False
-        return same_bits(self.flat[keep], self.flat0[keep])
+        """every entry no got() call covered still holds its initial bytes"""
+        view = {BF16: torch.int16, F32: torch.int32}[self.flat.dtype]
+        return not bool(((self.flat.view(view) != self.flat0.view(view)) & ~self.written).any())
 
 
 def run_gemm(ops, ck, tag, c, g):
-    """one tfx_gemm_store call described by c (the recorded / explicit geometry) on fresh operands, checked against float64"""
+    """one tfx_gemm_store call described by c (the recorded / explicit geometry) on fresh operands, checked against float64 in row chunks
+    of at most REF_VALUES outputs"""
     M, N, K, a_mn, b_mn, lda, ldb = c['M'], c['N'], c['K'], c['a_mn'], c['b_mn'], c['lda'], c['ldb']
     alpha, acc, ks, row_off = c['alpha'], c['acc'], c['ks'], c['row_off']
     A = operand(K if a_mn else M, M if a_mn else K, lda, g)
@@ -132,27 +143,34 @@ def run_gemm(ops, ck, tag, c, g):
     ops.gemm_store(A, lda, a_mn, B, ldb, b_mn, M, N, K, of.ptr if of else None, c['ld_f32'], ob.ptr if ob else None, c['ld_bf16'], bias, row_off,
                    alpha, acc, ks)
     _, kb, _, s = _lib.gemm_store_items(M, N, K, a_mn, b_mn, ks)
-    mag = abs(alpha) * (a64.abs() @ b64.abs().t())
-    ref = alpha * (a64 @ b64.t())
-    extra = torch.zeros_like(ref)
-    if bias is not None:
-        ref = ref + bias.double()
-        extra = extra + bias.double().abs()
-    E = c_acc(kb) * mag + (s + 2) * U24 * (mag + extra)
+    step = max(1, REF_VALUES // max(N, 1))
+    for r0 in range(0, M, step):
+        rs = slice(r0, min(r0 + step, M))
+        a = a64[rs]
+        mag = abs(alpha) * (a.abs() @ b64.abs().t())
+        ref = alpha * (a @ b64.t())
+        extra = mag
+        if bias is not None:
+            ref = ref + bias.double()
+            extra = mag + bias.double().abs()
+        E = c_acc(kb) * mag + (s + 2) * U24 * extra
+        if of is not None:
+            v = of.valid[rs]
+            want, Ef = ref[v], E[v]
+            if acc:
+                init = of.initial(rs)
+                want, Ef = want + init, Ef + (s + 2) * U24 * init.abs()
+            got = of.got(rs)
+            ck(f'{tag} fp32', got, want, Ef, row0 = int(of.valid[:r0].sum()))    # rows counted among the stored ones
+            rest = (got.double() - want).abs() - (Ef - c_acc(kb) * mag[v])
+            measured = (rest.clamp_min(0) / mag[v].clamp_min(1e-300)).max().item() if got.numel() else 0.
+            SHOWN['c_acc (measured) / C_ACC(kb)'] = max(SHOWN.get('c_acc (measured) / C_ACC(kb)', 0.), measured / c_acc(kb))
+            show_c_acc(SHOWN, kb, measured)
+        if ob is not None:
+            ck(f'{tag} bf16', ob.got(rs), ref, U8 * ref.abs() + (1 + U8) * E, row0 = r0)
     if of is not None:
-        v = of.valid
-        want, Ef = ref[v], E[v]
-        if acc:
-            want, Ef = want + of.initial(), Ef + (s + 2) * U24 * of.initial().abs()
-        got = of.got()
-        ck(f'{tag} fp32', got, want, Ef)
-        rest = (got.double() - want).abs() - (Ef - c_acc(kb) * mag[v])
-        measured = (rest.clamp_min(0) / mag[v].clamp_min(1e-300)).max().item() if got.numel() else 0.
-        SHOWN['c_acc (measured) / C_ACC(kb)'] = max(SHOWN.get('c_acc (measured) / C_ACC(kb)', 0.), measured / c_acc(kb))
-        SHOWN['c_acc (measured)'] = max(SHOWN.get('c_acc (measured)', 0.), measured)
         ck.true(f'{tag} fp32: bytes no row reaches untouched', of.rest_untouched())
     if ob is not None:
-        ck(f'{tag} bf16', ob.got(), ref, U8 * ref.abs() + (1 + U8) * E)
         ck.true(f'{tag} bf16: bytes no row reaches untouched', ob.rest_untouched())
 
 
@@ -185,7 +203,7 @@ def _record(calls, label, model, run):
 
 @pytest.fixture(scope = 'module')
 def recorded():
-    """every distinct gemm_store call of one eager forward + backward of four models"""
+    """every distinct gemm_store call of one eager forward + backward of seven models"""
     calls = {}
     # (a) d128, two modality types (dim_latent 32, 16), one modality instance: n_cond = 1
     torch.manual_seed(0)
@@ -218,14 +236,39 @@ def recorded():
                      dropout_key = fx['dropout_key'])
         total.backward()
     _record(calls, 'self-flow', w.student, selfflow)
+    # (e) d1536 with 8 heads of 64 and (f) d2048 with 16 heads of 128, the models of the wide training-step fixtures, on their two-modality
+    # batch: the dgrad du = dvg W1 over K = 2 Ip = 8192 / 11008, the W1 wgrad with 8192 / 11008 output rows through row_off
+    two_type_batch = lambda: synth.config4_batch(2, seed = 2, total_len = 300, dims = (32, 16), text_vocab = 64)
+    for name in ('small_wide1536', 'small_wide2048'):
+        fx = load_golden(name)
+        torch.manual_seed(0)
+        m = Transfusion(**fx['ctor'])
+        synth.fill_parameters_(m, seed = fx['seed'])
+        m = m.cuda().eval()
+        _record(calls, name[6:], m, lambda: m(two_type_batch(), times = fx['times']).backward())
+    # (g) dim_head 128, an odd head count and the learned value residual: the QKVG wgrad maps the mix rows at 3 HI + 4 (one pad row behind
+    # the 3 gate rows)
+    torch.manual_seed(0)
+    m = Transfusion(num_text_tokens = 64, dim_latent = 32, modality_default_shape = (4,), prob_uncond = 0.,
+                    transformer = dict(dim = 384, depth = 3, heads = 3, dim_head = 128, use_value_residual = True))
+    synth.fill_parameters_(m, seed = 8)
+    m = m.cuda().eval()
+    batch = synth.small_batch(3, seed = 1, dim_latent = 32, text_vocab = 64)
+    times = torch.rand(3, 3, generator = torch.Generator().manual_seed(5))             # up to 3 modality instances per sample
+    _record(calls, 'd384 h3x128 vres', m, lambda: m(batch, times = times).backward())
     torch.cuda.synchronize()
     return list(calls.values())
 
 
 def test_recorded_calls_keep_their_edge_cases(recorded):
     def has(pred):
-        return any(pred(c) for c in recorded)
+        return sorted({c['where'] for c in recorded if pred(c)})
     splits = lambda c: _lib.gemm_store_items(c['M'], c['N'], c['K'], c['a_mn'], c['b_mn'], c['ks'])[3]
+    kblocks = lambda c: _lib.gemm_store_items(c['M'], c['N'], c['K'], c['a_mn'], c['b_mn'], c['ks'])[1]
+
+    def lone_gap(r):
+        on = r >= 0
+        return bool((on[:-2] & ~on[1:-1] & on[2:]).any())
     want = {
         'K < 64': has(lambda c: c['K'] < 64),
         'N < 32': has(lambda c: c['N'] < 32),
@@ -235,7 +278,14 @@ def test_recorded_calls_keep_their_edge_cases(recorded):
         'a row offset not a multiple of 4': has(lambda c: c['row_off'] is not None and bool(((c['row_off'] >= 0) & (c['row_off'] % 4 != 0)).any())),
         'k_splits > 1': has(lambda c: splits(c) > 1),
         'bf16-only output': has(lambda c: c['bf16'] and not c['f32']),
+        'a dgrad (A K-major, B MN-major, no split) over more than 128 k-blocks and 256 token rows':
+            has(lambda c: not c['a_mn'] and c['b_mn'] and splits(c) == 1 and kblocks(c) > 128 and c['M'] >= 256),
+        'a wgrad with more than 8192 output rows through row_off, with -1 rows':
+            has(lambda c: c['row_off'] is not None and c['M'] > 8192 and bool((c['row_off'] == -1).any())),
+        'one -1 row between mapped rows (the mix rows behind an odd head count)': has(lambda c: c['row_off'] is not None and lone_gap(c['row_off'])),
     }
+    for k, v in want.items():
+        print(f'{k}: {", ".join(v)}')
     missing = [k for k, v in want.items() if not v]
     assert not missing, f'the recorded train steps no longer contain: {missing}'
 

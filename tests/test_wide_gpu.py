@@ -4,6 +4,11 @@
   bounds; their width lists stop at 1024): adaLN forward / backward with and without condition rows, the branch-gate backward, final RMSNorm
   forward / backward, token assemble / embedding backward / scatter-add / clean-flow rows, the Self-Flow cosine loss, and the
   AttentionResidual forward and deferred backward at depths that cross the 10-layer chunks of the backward assembly.
+- The fused GEMM epilogues and the GEGLU backward at both widths against float64, through the bodies of tests/test_block_epilogues_gpu.py
+  (same row count and bounds, the accumulator bound grown with the k-loop as helpers.c_acc states): gemm_resid in its attention-out,
+  text-only, FFN-out, bf16-only and U-Net skip forms, whose FFN-out and skip products run 48 to 86 k-blocks over 12 and 16 N tiles, at HI
+  below D (8 heads) and HI = D (32 heads); gemm_geglu with and without dropout over 64 and 86 value / gate tile pairs; geglu_bwd with and
+  without dropout at 512 and 704 threads per block, with the colsum_f32 bias sums.
 - Whole training steps against the reference's own outputs (oracle/make_golden_wide.py) at the parity bounds of tests/test_parity_gpu.py, the
   sampler against the reference under the greedy-margin rule, the captured `step_packed` graph against the eager step, and `torch.optim.Adam`
   steps against the fp32 checker."""
@@ -17,13 +22,18 @@ import test_aux_kernels_gpu as aux
 import test_block_epilogues_gpu as epi
 import test_norm_kernels_gpu as norm
 import test_selfflow_gpu as selfflow
-from helpers import compare_sampling, golden_noise, grad_fingerprint, load_golden, unpack_rows
+from helpers import cluster_mode, compare_sampling, golden_noise, grad_fingerprint, load_golden, unpack_rows  # noqa: F401  (cluster_mode: a fixture)
 from transfusion_pytorch_b200 import Transfusion, _lib, synth
 from transfusion_pytorch_b200.transfusion import MODEL_DIMS
 from oracle.dh128_reference import HeadDimOracleEngine
 
 pytestmark = pytest.mark.gpu
 WIDE = (1536, 2048)
+EPI_CONFIGS = [(1536, 8), (2048, 32)]                    # (D, H): HI = 64 H below D and equal to D
+# Measured on an H100 80GB HBM3 (700 W power limit), worst err / bound of the fused-epilogue checks at both widths: bf16 outputs 0.984 - 0.996
+# (the cast's rounding, which the bound states exactly); gemm_resid x_out 0.18 - 0.38 (the accumulator at 64 and 86 k-blocks: 7.0e-7 and
+# 7.4e-7 of |u| |W|^T); geglu_bwd dbias 0.012 - 0.014.  Per case: gemm_resid 0.1 s and +1.4 / +2.0 GiB of device memory at D = 1536 / 2048,
+# gemm_geglu 3.0 - 3.7 s and +4.3 / +5.8 GiB (its float64 reference in two row chunks), geglu_bwd 3.2 / 3.7 s and +6.4 / +8.6 GiB.
 LOSS_REL, HID_REL, GRAD_REL = 1e-3, 2e-2, 6e-2           # tests/test_parity_gpu.py
 MARGIN_BOUND, LATENT_TOL = 0.1, 5e-2                     # tests/test_dh128_gpu.py
 
@@ -88,6 +98,22 @@ def test_attn_residual_fwd_vs_float64(ops, D, L1):
 @pytest.mark.parametrize('depth', [1, 10, 11, 21, 64])
 def test_attn_residual_backward_vs_float64(ops, D, depth):
     ares.test_attn_residual_backward_vs_float64(ops, D, depth)
+
+
+# ------------------------------------------------------------------------------------------------ fused GEMM epilogues vs float64
+@pytest.mark.parametrize('D,H', EPI_CONFIGS, ids = [f'd{d}h{h}' for d, h in EPI_CONFIGS])
+def test_gemm_resid_vs_float64(ops, cluster_mode, D, H):
+    epi.test_gemm_resid_vs_float64(ops, cluster_mode, D, H, False)
+
+
+@pytest.mark.parametrize('D,H', EPI_CONFIGS, ids = [f'd{d}h{h}' for d, h in EPI_CONFIGS])
+def test_gemm_geglu_vs_float64(ops, cluster_mode, D, H):
+    epi.test_gemm_geglu_vs_float64(ops, cluster_mode, D, H, False)
+
+
+@pytest.mark.parametrize('D', WIDE)
+def test_geglu_bwd_vs_float64(ops, D):
+    epi.test_geglu_bwd_vs_float64(ops, D)
 
 
 # ------------------------------------------------------------------------------------------------ whole model
