@@ -60,8 +60,11 @@ int tfx_gemm_store(const void* A, long long lda, int a_mn_major, const void* B, 
  * gates fp32 [M][H] (logits); qk_inv fp32 [M][2H] (saved 1/|x| for backward).
  * kv_rows (optional, [M]): in-place kv-cache append - token m's post-RoPE key and its value are written to ROW kv_rows[m] of k / v, which
  * then point at one layer of the slab cache (replaces the cat / pad / stack of T.py:969-977, 2257-2277); q stays dense.
- * mix_pre (optional, fp32 [M][H], H <= 16): rows [3*H*64 + H, 3*H*64 + 2H) of W hold `to_learned_value_residual` (T.py:894-898); their products are
- * written here (pre-bias, pre-sigmoid). */
+ * mix_pre (optional, fp32 [M][H], any accepted H): rows [3*H*64 + H, 3*H*64 + 2H) of W hold `to_learned_value_residual` (T.py:894-898); their
+ * products are written here (pre-bias, pre-sigmoid).
+ * gates may be null (`Attention(gate_values = False)`, T.py:901-904, 1026-1027): no gate logits are written.  The 128 rows behind to_v (the gate
+ * tile: gate rows, mix rows, zero pad) exist iff gates or mix_pre is given: then W is [3*H*64 + 128][D] as above, otherwise [3*H*64][D] and the
+ * GEMM computes no gate tile. */
 int tfx_gemm_qkvg(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates, float* qk_inv,
                   const float* q_gamma, const float* k_gamma, const int* rope_pos, const float* rope_cs_t /* [32][rope_len][2], see tfx_rope_table */, int rope_len,
                   const int* kv_rows, float* mix_pre, void* stream);
@@ -70,7 +73,8 @@ int tfx_gemm_qkvg(const void* u, long long ldu, const void* W, long long ldw, in
  * mix_pre and the kv_rows append are those of tfx_gemm_qkvg (same accumulators, bit for bit). */
 int tfx_gemm_qkvg_rope(const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v, float* gates,
                        const int* rope_pos, const float* rope_cs_t, int rope_len, const int* kv_rows, float* mix_pre, void* stream);
-/* dim_head = 128 forms of the two: W = [to_qk | to_v | to_gates | pad], N = 3*H*128 + 128, one head per 128-column tile, so 1 <= H <= 16 (odd H too).
+/* dim_head = 128 forms of the two: W = [to_qk | to_v | gate tile], N = 3*H*128 + 128 (3*H*128 without gates and mix_pre, as above), one head per
+ * 128-column tile, so 1 <= H <= 16 (odd H too).
  * The qk-RMSNorm spans the head's 128 columns (scale sqrt(128)); RoPE takes 64 frequency pairs: rope_cs_t is [64][rope_len][2] (tfx_rope_table, n_freqs 64);
  * qk_inv is [M][2H] as above; q, k, v are [M][H*128]; gates are rows [3*H*128, +H) of W as in the 64-wide forms, the mix_pre rows start at the next
  * even row, 3*H*128 + H rounded up to even (so that an odd H keeps the bf16 pairs of their gradient 4-byte aligned). */
@@ -132,7 +136,8 @@ int tfx_attn_bwd_prep_d128(const void* do_gated, const void* o_gated, const floa
 int tfx_attn_bwd_d128(const void* q, const void* k, const void* v, const void* do_pre, long long ld_q, long long ld_k, long long ld_v, long long ld_do,
                       const float* lse, const float* dsum_hm, const int* kv_limit, const int* kt_kv0, const int* kt_kvend, const int* kt_q0, const int* kt_qend,
                       int n_kv_tiles, float* dq, float* dk, void* dv, long long ld_dv, int M, int H, float scale, float softcap, void* stream);
-/* backward of the qk-RMSNorm + RoPE epilogue; packs d[q | k | (v written by attn_bwd) | gates] bf16 [M][out_ld] */
+/* backward of the qk-RMSNorm + RoPE epilogue; packs d[q | k | (v written by attn_bwd) | gates] bf16 [M][out_ld].  gates null (ungated model):
+ * no gate-gradient column is written and dsum_mh is not read (may be null).  The same holds for the three packs below. */
 int tfx_qk_bwd_pack(const float* dq, const float* dk, const void* q_bf16, const void* k_bf16, const float* qk_inv, const float* q_gamma, const float* k_gamma,
                     const int* rope_pos, const float* rope_cs, const float* gates, const float* dsum_mh, void* dqkvg_bf16, long long out_ld,
                     float* dq_gamma, float* dk_gamma, int M, int H, void* stream);

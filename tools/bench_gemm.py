@@ -48,6 +48,9 @@ def main():
     cases = {   # name: (launch, algorithmic FLOPs, outputs to dump)
         'qkvg   [131072 x 1664 x 512]': (lambda: ops.gemm_qkvg(u, D, wq, D, M, H, D, q, k, v, gates, qk_inv, gq, gk, pos, rope_tt, 1024, None, None),
                                          2.0 * M * NQ * D, dict(q = q, k = k, v = v, gates = gates, qk_inv = qk_inv)),
+        # `gate_values = False` without the value residual: no gate tile (N = 3 HI)
+        'qkvg ungated [131072 x 1536 x 512]': (lambda: ops.gemm_qkvg(u, D, wq, D, M, H, D, q, k, v, None, qk_inv, gq, gk, pos, rope_tt, 1024, None, None),
+                                               2.0 * M * 3 * HI * D, dict(q = q, k = k, v = v, qk_inv = qk_inv)),
         'resid  [131072 x 512 x 512]': (lambda: ops.gemm_resid(att, HI, None, 0, 0, wo, HI, M, D, HI, None, x_a, x_b, None, yA, cond_row, zg[:, D:], 2 * D, ls),
                                         2.0 * M * D * HI, dict(x_out = x_b, y = yA)),
         'resid  [131072 x 512 x 1408]': (lambda: ops.gemm_resid(h, Ip, None, 0, 0, w2r, Ip, M, D, Ip, bias2, x_b, None, x_cb, yF, cond_row, zg[:, :D], 2 * D, ls),

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Cost of model options in the resident training step, on the path bench.py times (`DataParallelTrainer.step_packed`, CUDA-graph replay).
 Each positional argument is one arm, WIDTHxDEPTHxBATCH[:key=value,...] with BATCH in 1024-token samples; the keys are `dim_head` (default 64),
-`heads` (default width // dim_head), `qk_rmsnorm` (0 / 1), `dropout` (`ff_kwargs = dict(dropout = p)`), `recon` (`reconstruction_loss_weight`)
-and `data` (config2, the default, or config4).  Each arm runs in a process of its own, so its device memory is returned before the next
+`heads` (default width // dim_head), `qk_rmsnorm` (0 / 1), `gated` (0 / 1: `attn_kwargs = dict(gate_values = ...)`), `vres` (0 / 1:
+`use_value_residual`), `dropout` (`ff_kwargs = dict(dropout = p)`), `recon` (`reconstruction_loss_weight`) and `data` (config2, the default,
+or config4).  Each arm runs in a process of its own, so its device memory is returned before the next
 starts, and the arms alternate in the order given for --rounds rounds.  Prints the card, its power limit and max SM clock once, then per arm
 the median and minimum step time of --steps replays, tokens, tokens/s, peak device memory and the SM clock after the arm.
 
@@ -12,6 +13,7 @@ and `ares_bytes_per_token` below, over event time).  A launch shorter than the h
 time, so there the ms are upper bounds and the GB/s lower bounds.
 
     python tools/bench_step.py 512x8x128 512x8x128:qk_rmsnorm=0 --kernels
+    python tools/bench_step.py 512x8x128 512x8x128:gated=0 2048x8x16:heads=32 2048x8x16:heads=32,vres=1
     python tools/bench_step.py 512x8x128:data=config4 512x8x128:data=config4,recon=0.1"""
 import argparse, os, subprocess, sys
 import torch
@@ -20,7 +22,7 @@ from transfusion_pytorch_b200 import Transfusion, synth
 from transfusion_pytorch_b200.data_parallel import DataParallelTrainer
 from transfusion_pytorch_b200.modality_processing import pack_batch
 
-KEYS = ('dim_head', 'heads', 'qk_rmsnorm', 'dropout', 'recon', 'data')
+KEYS = ('dim_head', 'heads', 'qk_rmsnorm', 'gated', 'vres', 'dropout', 'recon', 'data')
 DATA = {'config2': dict(dim_latent = 384, modality_default_shape = (256,)),
         'config4': dict(dim_latent = (384, 192), modality_default_shape = ((4,), (2,)))}
 CHUNK = 10                    # later layers per deferred-assembly launch (rowops.cu BWD2_CHUNK)
@@ -36,10 +38,15 @@ def parse_arm(spec):
         raise ValueError(f'{spec}: unknown key(s) {sorted(set(kv) - set(KEYS))}; the keys are {", ".join(KEYS)}')
     dim_head = int(kv.get('dim_head', 64))
     tr = dict(dim = D, depth = depth, dim_head = dim_head, heads = int(kv.get('heads', D // dim_head)))
+    for key in ('qk_rmsnorm', 'gated', 'vres'):
+        if key in kv and kv[key] not in ('0', '1'):
+            raise ValueError(f'{spec}: {key} is 0 or 1')
     if 'qk_rmsnorm' in kv:
-        if kv['qk_rmsnorm'] not in ('0', '1'):
-            raise ValueError(f'{spec}: qk_rmsnorm is 0 or 1')
         tr['qk_rmsnorm'] = kv['qk_rmsnorm'] == '1'
+    if 'gated' in kv:
+        tr['attn_kwargs'] = dict(gate_values = kv['gated'] == '1')
+    if 'vres' in kv:
+        tr['use_value_residual'] = kv['vres'] == '1'
     if 'dropout' in kv:
         tr['ff_kwargs'] = dict(dropout = float(kv['dropout']))
     data = kv.get('data', 'config2')

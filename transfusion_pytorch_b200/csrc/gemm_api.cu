@@ -32,8 +32,10 @@ static int dispatch_major(const GemmOperand& A, const GemmOperand& B, const Gemm
   return launch_gemm_t<true, false, EPI_STORE>(A, B, p, sms, st);
 }
 
-// the four tfx_gemm_qkvg* entry points; `name` is the entry point's name for error messages.  W is [to_qk | to_v | to_gates | pad]
-// with N = 3 H DH + 128.  At DH = 64 a 128-column tile holds two heads, so H is even; at 128 it holds one, so any H in [1, 16].
+// the four tfx_gemm_qkvg* entry points; `name` is the entry point's name for error messages.  W is [to_qk | to_v | gate tile] with
+// N = 3 H DH + 128, the 128-row gate tile holding to_gates (rows [0, H)) and the value-residual mix (rows [round_even(H), + H)); with
+// neither gates nor mix_pre there is no gate tile and N = 3 H DH.  At DH = 64 a 128-column tile holds two heads, so H is even; at 128 it
+// holds one, so any H in [1, 16].
 template <int EPI>
 static int gemm_qkvg(const char* name, const void* u, long long ldu, const void* W, long long ldw, int M, int H, int D, void* q, void* k, void* v,
                      float* gates, float* qk_inv, const float* q_gamma, const float* k_gamma, const int* rope_pos, const float* rope_cs_t, int rope_len,
@@ -41,14 +43,13 @@ static int gemm_qkvg(const char* name, const void* u, long long ldu, const void*
   constexpr int DH = qkvg_dh(EPI);
   if (M <= 0) return 0;
   if constexpr (DH == 64) {
-    TFX_REQUIRE(!mix_pre || H <= 16, "%s: the value-residual mix columns share the 32-column gate slab: heads must be <= 16 (got %d)", name, H);
     TFX_REQUIRE(H >= 2 && H % 2 == 0 && H <= 32, "%s: heads must be even and in [2, 32] (got %d)", name, H);
   } else {
     TFX_REQUIRE(H >= 1 && H <= 16, "%s: heads must be in [1, 16] (got %d)", name, H);
   }
   TFX_REQUIRE(ldu % 8 == 0 && ldw % 8 == 0, "%s: row pitches must be multiples of 8", name);
   GemmParams p; memset(&p, 0, sizeof(p));
-  p.M = M; p.N = 3 * H * DH + 128; p.K = D; p.k_splits = 1; p.H = H;
+  p.M = M; p.N = 3 * H * DH + (gates || mix_pre ? 128 : 0); p.K = D; p.k_splits = 1; p.H = H;
   p.q = (__nv_bfloat16*)q; p.k = (__nv_bfloat16*)k; p.v = (__nv_bfloat16*)v; p.gates = gates; p.qk_inv = qk_inv;
   p.q_gamma = q_gamma; p.k_gamma = k_gamma; p.rope_pos = rope_pos; p.rope_cs = (const float2*)rope_cs_t; p.rope_len = rope_len; p.kv_rows = kv_rows; p.mix_pre = mix_pre;
   GemmOperand a{u, ldu, false}, b{W, ldw, false};

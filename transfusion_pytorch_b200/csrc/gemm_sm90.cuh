@@ -61,9 +61,9 @@ struct GemmParams {
   // ---- EPI_QKVG* at head dim DH = 64 or 128 (N tile 128 = 128 / DH heads: H DH / 128 q tiles | as many k | as many v | 1 gate tile)
   int H;                       // heads (even at DH = 64)
   __nv_bfloat16 *q, *k, *v;    // [M][H*DH]
-  float* gates;                // [M][H]   raw gate logits
+  float* gates;                // [M][H]   raw gate logits; null for an ungated model (columns [0, H) of the gate tile are then unused)
   float* mix_pre;              // [M][H]   optional: columns [m0, m0 + H) of the gate tile, m0 = H rounded up to even, = pre-activation of the
-                               //          learned value-residual mix (T.py:956-960)
+                               //          learned value-residual mix (T.py:956-960).  Without both there is no gate tile (N = 3 H DH)
   float* qk_inv;               // [M][2H]  1/max(|x|,eps) for q heads then k heads
   const float *q_gamma, *k_gamma;   // [DH]
   const int* rope_pos;         // [M]
@@ -655,9 +655,11 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           acc_ld32(acc, erow, 0, r);
           if (row_ok) {
             constexpr int H_MAX = DH == 64 ? 32 : 16;   // the largest head count the entry points accept at this width
-            float* dst = p.gates + (long long)row * p.H;
+            if (p.gates) {                              // null for an ungated model (`gate_values = False`), whose tile carries the mix only
+              float* dst = p.gates + (long long)row * p.H;
 #pragma unroll
-            for (int j = 0; j < H_MAX; ++j) if (j < p.H) dst[j] = __uint_as_float(r[j]);
+              for (int j = 0; j < H_MAX; ++j) if (j < p.H) dst[j] = __uint_as_float(r[j]);
+            }
             if (p.mix_pre) {                            // mix columns start at an even column (bf16 pairs of their gradient stay 4-byte aligned)
               const int m0 = (p.H + 1) & ~1;
               float* dm = p.mix_pre + (long long)row * p.H;
@@ -667,6 +669,15 @@ gemm_sm90_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 // column at 64, the rounded start computed once at 128.
                 const int mj = DH == 64 ? p.H : m0;
                 if (j >= mj && j < mj + p.H) dm[j - mj] = __uint_as_float(r[j]);
+              }
+              // above 16 heads of 64 the mix runs past the first slice, into columns [32, 2 H): loaded into the same words once the
+              // first slice is stored, so no more accumulators are live than at H <= 16 (at 128, H <= 16 keeps it in the first slice)
+              if constexpr (DH == 64) {
+                if (p.H > 16) {
+                  acc_ld32(acc, erow, 32, r);
+#pragma unroll
+                  for (int j = 0; j < 32; ++j) if (32 + j < 2 * p.H) dm[32 + j - p.H] = __uint_as_float(r[j]);
+                }
               }
             }
           }

@@ -1063,7 +1063,8 @@ __global__ void __launch_bounds__(ROW_THREADS) clean_flow_bwd_k(float* __restric
 // (T.py:950-965).  !NORM (EPI_QKVG_ROPE): q = R(pos) x, so d x = R(pos)^T d q per interleaved pair; no saved values and no gammas are needed.
 // One warp per token; DH / 8 lanes share a head (8 at DH = 64, 16 at 128) and a lane owns 8 consecutive dims = 4 rope pairs (32 B fp32 /
 // 16 B bf16 accesses), so a warp covers 32 / (DH / 8) heads per pass and the per-head dot product is a log2(DH / 8)-step shuffle.
-// rope_cs is [pos][DH / 2] (cos, sin).  Without NORM, q, k, qk_inv, the gammas and their gradients are not read and may be null.
+// rope_cs is [pos][DH / 2] (cos, sin).  Without NORM, q, k, qk_inv, the gammas and their gradients are not read and may be null.  Without
+// gates (`gate_values = False`) neither is dsum, and no gate column is written.
 // xhat is rebuilt from the bf16 output as R^T q / (sqrt(DH) (gamma + 1)): where gamma_j = -1 the forward wrote y_j = 0 and xhat_j is lost, so
 // dx_j and dgamma_j come out 0 instead of -inv xhat_j (xhat . dxhat) and sum sqrt(DH) dy_j xhat_j; near -1 the bf16 error of the rope partner
 // is amplified by |gamma_partner + 1| / |gamma_j + 1|.
@@ -1151,8 +1152,8 @@ __global__ void __launch_bounds__(ROW_THREADS) qk_bwd_pack_k(const float* __rest
         if (act) *reinterpret_cast<uint4*>(out + (long long)row * out_ld + which * HI + h * DH + sub * 8) = make_uint4(w[0], w[1], w[2], w[3]);
       }
     }
-    // gate logits: d g = (1 - sigmoid(g)) * sum_d dO_gated * O_gated
-    if (lane < H) {
+    // gate logits: d g = (1 - sigmoid(g)) * sum_d dO_gated * O_gated; an ungated model (gates null) has no gate column
+    if (gates && lane < H) {
       const float gl = gates[(long long)row * H + lane];
       const float sg = 1.f / (1.f + __expf(-gl));
       out[(long long)row * out_ld + 3 * HI + lane] = __float2bfloat16((1.f - sg) * dsum[(long long)row * H + lane]);

@@ -153,16 +153,22 @@ class Engine:
         self.HI = self.H * self.DH
         self.inner = tr.ff_inner
         self.Ip = _round_up(self.inner, 64)
-        self.NQ = 3 * self.HI + 128                 # packed rows of [to_qk | to_v | to_gates | pad]
-        # first packed row of the value-residual mix Linear (in the pad): right behind the gates, at an even row so that the bf16 pairs of
-        # its gradient columns stay 4-byte aligned (an odd head count exists at dim_head 128 only)
+        self.laser, self.laser_clamp, self.vres = tr.attn_laser, tr.laser_softclamp_value, tr.use_value_residual
+        # `attn_kwargs = dict(gate_values = False)` (T.py:901-904, 1026-1027): no to_gates, attention output without the sigmoid(gate) factor;
+        # every attention-side call of such a model gets gates = None
+        self.gated = bool(getattr(tr, 'gate_values', True))
+        # packed rows [to_qk | to_v | gate tile]: the 128-row gate tile (to_gates at rows [0, H), the value-residual mix Linear at
+        # [round_even(H), + H), zero pad) exists iff the model is gated or has the value residual; otherwise the QKVG GEMM computes no tile
+        self.gate_tile = self.gated or self.vres
+        self.NQ = 3 * self.HI + (128 if self.gate_tile else 0)
+        # first packed row of the mix Linear: behind the gates, at an even row so that the bf16 pairs of its gradient columns stay 4-byte aligned
+        # (an odd head count exists at dim_head 128 only)
         self.MIX = 3 * self.HI + _round_up(self.H, 2)
         self.V = model.text_embed.weight.shape[0]
         self.Vp = _round_up(self.V, 8)
         self.Kt = _round_up(self.D + 1, 64)         # padded K of the time-cond Linear
         self.W = 2 * self.depth                     # AdaptiveWrappers
         self.softcap = tr.softcap_value
-        self.laser, self.laser_clamp, self.vres = tr.attn_laser, tr.laser_softclamp_value, tr.use_value_residual
         # qk_rmsnorm = False (T.py:949-951 skipped): q, k are RoPE(u W^T) only, so no bound on the logits follows from the gammas and every layer runs
         # the general (running-maximum) attention kernels; the q / k norm gammas stay out of the flat buffers (their .grad stays None, as in the reference)
         self.qk_norm = bool(getattr(tr, 'qk_rmsnorm', True))
@@ -276,11 +282,12 @@ class Engine:
             b1_off = self.offs[f'{pre}.2.fn.net.0.bias']
             w1_rows = torch.where(self.w1_row_src64 >= 0, w1_off + self.w1_row_src64 * D, torch.full_like(self.w1_row_src64, -1))
             b1_cols = torch.where(self.w1_row_src64 >= 0, b1_off + self.w1_row_src64, torch.full_like(self.w1_row_src64, -1)).to(I32)
-            q_off, v_off, g_off = self.offs[f'{pre}.1.fn.to_qk.0.weight'], self.offs[f'{pre}.1.fn.to_v.0.weight'], self.offs[f'{pre}.1.fn.to_gates.0.weight']
-            r = np.full(self.NQ, -1, dtype = np.int64)
+            q_off, v_off = self.offs[f'{pre}.1.fn.to_qk.0.weight'], self.offs[f'{pre}.1.fn.to_v.0.weight']
+            r = np.full(self.NQ, -1, dtype = np.int64)              # -1: a packed row without a parameter (pad, or the gates of an ungated model)
             r[:2 * HI] = q_off + np.arange(2 * HI) * D
             r[2 * HI:3 * HI] = v_off + np.arange(HI) * D
-            r[3 * HI:3 * HI + H] = g_off + np.arange(H) * D
+            if self.gated:
+                r[3 * HI:3 * HI + H] = self.offs[f'{pre}.1.fn.to_gates.0.weight'] + np.arange(H) * D
             if f'{pre}.1.fn.to_learned_value_residual.0.weight' in self.offs:        # value-residual mix Linear: pad rows [MIX, MIX + H) of the packed weight
                 r[self.MIX:self.MIX + H] = self.offs[f'{pre}.1.fn.to_learned_value_residual.0.weight'] + np.arange(H) * D
             w2_off = self.offs[f'{pre}.2.fn.net.3.weight']
@@ -335,7 +342,8 @@ class Engine:
             wq = dst(f'qkvg{i}', self.NQ, D)
             job(self.P(f'{pre}.1.fn.to_qk.0.weight'), D, D, None, wq, 2 * HI, D)
             job(self.P(f'{pre}.1.fn.to_v.0.weight'), D, D, None, wq[2 * HI:], HI, D)
-            job(self.P(f'{pre}.1.fn.to_gates.0.weight'), D, D, None, wq[3 * HI:], H, D)
+            if self.gated:
+                job(self.P(f'{pre}.1.fn.to_gates.0.weight'), D, D, None, wq[3 * HI:], H, D)
             if f'{pre}.1.fn.to_learned_value_residual.0.weight' in self.named:
                 job(self.P(f'{pre}.1.fn.to_learned_value_residual.0.weight'), D, D, None, wq[self.MIX:], H, D)
             job(self.P(f'{pre}.1.fn.to_out.1.weight'), HI, HI, None, dst(f'wo{i}', D, HI), D, HI)
@@ -570,7 +578,7 @@ class Engine:
             else:
                 # inference shares one buffer set across layers, but the value residual reads the FIRST layer's values in every later layer
                 k = self.buf(f'{lt}k', (M, HI), BF16); v = self.buf(f'{lt}v0' if (self.vres and i == 0) else f'{lt}v', (M, HI), BF16)
-            gates = self.buf(f'{lt}g', (M, H), F32)
+            gates = self.buf(f'{lt}g', (M, H), F32) if self.gated else None
             has_mix = self.vres and i > 0
             mixpre = self.buf(f'{lt}mix', (M, H), F32) if has_mix else None
             if self.qk_norm:
@@ -918,15 +926,17 @@ class Engine:
             dog = self.buf('dog', (M, HI), BF16)
             o.gemm_store(dy, D, 0, pk[f'wo{i}'], HI, 1, M, HI, D, None, 0, dog, HI, None, None, 1.0, 0, 1)
             wgrad(dy, D, D, L['att'], HI, HI, f'{pre}.1.fn.to_out.1.weight')
-            dop = self.buf('dop', (M, HI), BF16); dsum_hm = self.buf('dsum_hm', (H, M), F32); dsum_mh = self.buf('dsum_mh', (M, H), F32)
+            dop = self.buf('dop', (M, HI), BF16); dsum_hm = self.buf('dsum_hm', (H, M), F32); dsum_mh = self.buf('dsum_mh', (M, H), F32) if self.gated else None
             dq = self.buf('dq', (M, HI), F32); dk = self.buf('dk', (M, HI), F32)
             if self.laser:
                 getattr(o, 'laser_bwd_prep' + self.sfx)(dog, L['o_l'], L['gates'], dop, dsum_hm, dsum_mh, dq, M, H)
             else:
                 getattr(o, 'attn_bwd_prep' + self.sfx)(dog, L['att'], L['gates'], dop, dsum_hm, dsum_mh, dq, M, H)
             dqkvg = self.buf('dqkvg', (M, self.NQ), BF16)
-            if i == self.depth - 1:
-                dqkvg[:, 3 * HI + H:].zero_()   # pad columns are never written by the kernels; cleared once per backward (inside captured graphs too)
+            if i == self.depth - 1 and self.gate_tile:
+                # pad columns (and the gate columns of an ungated model) are never written by the kernels; cleared once per backward (inside
+                # captured graphs too)
+                dqkvg[:, 3 * HI + (H if self.gated else 0):].zero_()
             fp = self.fastp[i] if self.fast else None
             if self.fast:
                 o.attn_bwd_tc(L['q'], L['k'], L['v_att'], dop, HI, HI, HI, HI, L['lse'], dsum_hm, dv['kv_limit'], dv['k2_kv0'], dv['k2_kvend'], dv['k2_q0'], dv['k2_qend'],

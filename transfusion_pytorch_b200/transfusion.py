@@ -32,7 +32,8 @@ from .modality_processing import (
 MAX_DEPTH = 64
 # Model widths the row kernels are built for: the cases of TFX_DISPATCH_NCH (csrc/common.cuh), D = 128 * NCH
 MODEL_DIMS = (128, 256, 384, 512, 768, 1024, 1536, 2048)
-# Heads the attention kernels take: two 64-wide heads per 128-column GEMM tile, at most 32 (gemm_qkvg's 32-column gate slab)
+# Heads the attention kernels take at dim_head 64: two heads per 128-column GEMM tile, at most 32 (an inner width of 2048, the widest the
+# q / k backward pack and the row attention kernels are built for)
 MIN_HEADS, MAX_HEADS = 2, 32
 DIM_HEADS = (64, 128)                # attention head widths the kernels implement
 MAX_HEADS_D128 = 16                  # heads at dim_head = 128 (inner width <= 2048, as at 64)
@@ -146,7 +147,7 @@ class _Fourier(Module):
 
 
 class _AttentionParams(Module):
-    def __init__(self, dim, dim_head, heads, learned_value_residual_mix = False):
+    def __init__(self, dim, dim_head, heads, learned_value_residual_mix = False, gate_values = True):
         super().__init__()
         inner = dim_head * heads
         if learned_value_residual_mix:           # T.py:894-898 (layers after the first, `use_value_residual`)
@@ -154,7 +155,8 @@ class _AttentionParams(Module):
         self.to_qk = nn.Sequential(nn.Linear(dim, inner * 2, bias = False))
         self.q_norm, self.k_norm = _Gamma(dim_head), _Gamma(dim_head)
         self.to_v = nn.Sequential(nn.Linear(dim, inner, bias = False))
-        self.to_gates = nn.Sequential(nn.Linear(dim, heads, bias = False))
+        if gate_values:                          # T.py:901-904: `gate_values = False` builds no to_gates
+            self.to_gates = nn.Sequential(nn.Linear(dim, heads, bias = False))
         self.to_out = nn.Sequential(nn.Identity(), nn.Linear(inner, dim, bias = False))
 
 
@@ -226,8 +228,7 @@ class Transformer(Module):
         # attention dropout (T.py:1017) is not implemented by the attention kernels.  With use_flex_attn the reference takes the flex_attention
         # branch on CUDA (T.py:987-995), which applies no attention dropout, so there `dropout` is accepted and has no effect.
         if dropout != 0. and not use_flex_attn: unsupported.append('dropout > 0 (attention dropout) without use_flex_attn')
-        if use_value_residual and heads > 16: unsupported.append('use_value_residual with heads > 16')
-        extra = set(attn_kwargs) - {'softcap_value', 'laser_softclamp_value'}
+        extra = set(attn_kwargs) - {'softcap_value', 'laser_softclamp_value', 'gate_values'}
         if extra: unsupported.append(f'attn_kwargs {sorted(extra)}')
         extra = set(ff_kwargs) - {'dropout'}         # FeedForward(dim, mult, dropout) (T.py:837-850): dropout is its only option besides the two above
         if extra: unsupported.append(f'ff_kwargs {sorted(extra)}')
@@ -240,6 +241,7 @@ class Transformer(Module):
         self.qk_rmsnorm = bool(qk_rmsnorm)           # False: q, k = RoPE(to_qk(x)) without the norms (T.py:949-951); their gammas stay built (T.py:886-888)
         self.laser_softclamp_value = float(attn_kwargs.get('laser_softclamp_value', 15.))
         self.softcap_value = float(attn_kwargs.get('softcap_value', 50.))
+        self.gate_values = bool(attn_kwargs.get('gate_values', True))      # False: out = to_out(attn v), no sigmoid(gate) factor (T.py:1026-1027)
         self.ff_inner = int(dim * ff_expansion_factor * 2 / 3)
         self.ff_dropout = ff_dropout                 # nn.Dropout after GEGLU (T.py:848): fused into the GEGLU GEMM epilogue, training forwards only
 
@@ -247,7 +249,8 @@ class Transformer(Module):
         layers = ModuleList([])
         for ind in range(depth):
             skip_proj = nn.Linear(dim * 2, dim, bias = False) if (ind >= depth / 2 and unet_skips) else None
-            attn = _AdaptiveParams(_AttentionParams(dim, dim_head, heads, learned_value_residual_mix = ind > 0 and use_value_residual), dim, dim * 4)
+            attn = _AdaptiveParams(_AttentionParams(dim, dim_head, heads, learned_value_residual_mix = ind > 0 and use_value_residual,
+                                                    gate_values = self.gate_values), dim, dim * 4)
             ff = _AdaptiveParams(_FeedForwardParams(dim, self.ff_inner), dim, dim * 4)
             layers.append(ModuleList([skip_proj, attn, ff, _AttnResidualParams(dim)]))
         self.layers = layers
